@@ -1,6 +1,7 @@
-"""Benchmark of the RigL hot path: sparse train step (+ the periodic mask update) on B200.
+"""Benchmark of the RigL hot path: sparse train step (+ the periodic mask update) on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--config c2|c3|c4|c5] [--impl ours|reference]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Configs (BASELINE.json `configs`; the metric is quoted on c2, the default):
@@ -11,7 +12,9 @@ Configs (BASELINE.json `configs`; the metric is quoted on c2, the default):
 All: RigL, drop fraction 0.3 cosine, update every 100 steps, Nesterov momentum, weak scaling (fixed per-GPU
 batch).  The timed region always contains ceil(steps/100) mask updates (the schedule is aligned so that the
 first one falls in the middle of the region), so `value` includes their cost at the reference's own cadence
-or denser.  One JSON line on rank 0: the driver contract plus `roofline`, `cpu_baseline`, `mask_update_ms`.
+or denser.  One JSON line on rank 0: the result plus `roofline`, `cpu_baseline`, `mask_update_ms`.
+--dump-outputs DIR writes what the last timed step computed (see dump_outputs) as DIR/<name>.npy; the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -46,31 +49,14 @@ UPDATE_EVERY = 100
 
 
 def _peaks():
+  """HBM bandwidth (GB/s) and dense bf16 rate (TFLOP/s) the roofline fractions are taken against: MEASURED_PEAKS.json
+  when present, else NVIDIA's data-sheet figures for the H100 SXM (700 W) -- an upper bound, not a measured rate."""
   path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
   if os.path.exists(path):
     with open(path) as f:
       d = json.load(f)
-    return d.get('hbm_gbs', 6650.0), d.get('bf16_tflops_sustained', 1400.0), 'measured'
-  return 6650.0, 1400.0, 'fallback'
-
-
-def _recorded_traffic(cfg_name):
-  """DRAM bytes per step of the conv kernel family from the committed ncu pass of the SAME workload
-  (profiles/*_dram_traffic_step.json: dram__bytes_read.sum + dram__bytes_write.sum, c2 at batch 256).  ncu
-  cannot run inside a timed bench, so this is the recorded capture, not a live measurement; null for the
-  configs that have no capture."""
-  if cfg_name != 'c2':
-    return None
-  for name in ('r02_dram_traffic_step.json', 'r01_dram_traffic_step.json'):
-    path = os.path.join(ROOT, 'profiles', name)
-    try:
-      with open(path) as f:
-        d = json.load(f)
-      return {'dram_bytes_per_step': d['conv_family_dram_bytes_per_step'], 'launches': d['conv_family_launches'],
-              'source': 'profiles/' + name + ' (recorded ncu capture, not measured by this run)'}
-    except Exception:
-      continue
-  return None
+    return d.get('hbm_gbs', 3350.0), d.get('bf16_tflops_sustained', 989.0), 'measured'
+  return 3350.0, 989.0, 'datasheet'
 
 
 class ClockSampler(object):
@@ -174,6 +160,27 @@ def masked_flops_per_image(model, image, dev):
           'algorithmic_gflop': (2 * f_s + f_d - first_s) / 1e9, 'dense_executed_gflop': (3 * f_d - first_d) / 1e9}
 
 
+DUMP_SAMPLES = 1 << 22           # per sampled array: 16 MB of float32
+
+
+def dump_outputs(model, loss, out_dir):
+  """Writes what the timed path hands its caller after a step: the loss, and -- the model being too large to store
+  whole -- the same fixed, seeded sample of the masked layers' weights, masks and dense gradients (all masked layers
+  concatenated in registry order).  float32 .npy files, 48 MB in all."""
+  os.makedirs(out_dir, exist_ok=True)
+  layers = model.registry.layers()
+  flat = lambda ts: torch.cat([t.detach().reshape(-1).float() for t in ts])
+  weights = flat(l.weight for l in layers)
+  masks = flat(l.mask.to_dense() for l in layers)
+  grads = flat(l.masked_weights.dense_grad for l in layers)
+  n = weights.numel()
+  idx = np.sort(np.random.RandomState(0).choice(n, size=min(n, DUMP_SAMPLES), replace=False))
+  idx = torch.from_numpy(idx).to(weights.device)
+  np.save(os.path.join(out_dir, 'loss.npy'), np.asarray([float(loss.detach().float().item())], np.float32))
+  for name, t in (('weights_sample', weights), ('masks_sample', masks), ('dense_grads_sample', grads)):
+    np.save(os.path.join(out_dir, name + '.npy'), t[idx].cpu().numpy().astype(np.float32))
+
+
 def run_ours(args):
   from rigl_b200 import _cabi
   from rigl_b200 import workloads
@@ -235,8 +242,9 @@ def run_ours(args):
   start.record()
   marks[0].record()
   n_updates, update_steps = 0, []
+  loss = None
   for i in range(args.steps):
-    harness.step(images, labels)
+    loss = harness.step(images, labels)
     marks[i + 1].record()
     if harness.opt.last_update_was_mask_update:
       n_updates += 1
@@ -245,6 +253,8 @@ def run_ours(args):
   barrier()
   per_step = [marks[i].elapsed_time(marks[i + 1]) for i in range(args.steps)]
   clocks = sampler.stop() if rank == 0 else None
+  if args.dump_outputs and rank == 0 and loss is not None:     # after the clock samples: the GPU idles meanwhile
+    dump_outputs(model, loss, args.dump_outputs)
   launches = _cabi.launch_count() + getattr(harness, 'replayed_kernel_launches', 0) - launches0
   ms = torch.tensor([start.elapsed_time(stop)], device=dev, dtype=torch.float64)
   if dist is not None:
@@ -353,7 +363,7 @@ def run_ours(args):
       'config': {'workload': cfg['workload'] + ', RigL drop 0.3 cosine every 100 steps, Nesterov momentum',
                  'name': args.config, 'global_batch': batch * world, 'per_gpu_batch': batch,
                  'parallelism': 'dp%d' % world,
-                 'l2_policy': 'inputs larger than L2 (activations per step >> 126 MB)',
+                 'l2_policy': 'inputs larger than L2 (activations per step >> 50 MB)',
                  'mask_updates_in_timed_region': n_updates, 'mask_update_steps': update_steps,
                  'step_ms': {'p50': float(np.median(per_step)), 'p90': float(np.percentile(per_step, 90)),
                              'max': float(max(per_step)), 'argmax': int(np.argmax(per_step)),
@@ -368,7 +378,7 @@ def run_ours(args):
       'mask_update_ms': mask_ms,
       'mask_update_algorithmic_GBps': 8.25 * total_w / mask_ms / 1e6,
       'roofline': {'bound': 'tensor',
-                   'kernel': 'k_igemm_kmajor2 / k_igemm_wgrad / k_halo3x3_* / k_stem_s2d_* (all masked conv+linear launches)',
+                   'kernel': 'k_igemm_kmajor / k_igemm_wgrad / k_halo3x3_* / k_stem_s2d_* (all masked conv+linear launches)',
                    'achieved': achieved_tf, 'peak': tf_peak, 'unit': 'TFLOP/s', 'frac': achieved_tf / tf_peak,
                    # the metric's own fraction: masked FLOPs of the whole job over the whole step (all kernels)
                    'achieved_step': step_tf, 'frac_step': step_tf / (tf_peak * world),
@@ -377,7 +387,7 @@ def run_ours(args):
                    'dense_executed_gflop_per_image': flops['dense_executed_gflop'],
                    'dense_executed_tflops': flops['dense_executed_gflop'] * batch / conv_ms,
                    'conv_ms_per_step': conv_ms, 'conv_launches_per_step': n_conv_launch,
-                   'ms_per_step_by_kind': per_kind, 'traffic': _recorded_traffic(args.config)},
+                   'ms_per_step_by_kind': per_kind},
   }
   if world == 1 and not args.no_cpu_baseline:
     out['cpu_baseline'] = cpu_baseline_leg(args.config, sample_batch=args.cpu_batch)
@@ -512,8 +522,11 @@ def main():
   ap.add_argument('--no-cpu-baseline', action='store_true')
   ap.add_argument('--layer-report', default=None)
   ap.add_argument('--no-graph', action='store_true', help='run the step eagerly (no CUDA-graph replay)')
+  ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                  help='write the loss and a seeded sample of the weights, masks and dense gradients after the last '
+                       'timed step as DIR/<name>.npy')
   ap.add_argument('--scaling', default='weak', choices=['weak', 'strong'],
-                  help='weak (default, the driver contract): the per-GPU batch is fixed; strong: the GLOBAL batch of '
+                  help='weak (default): the per-GPU batch is fixed; strong: the GLOBAL batch of '
                        'the config is fixed and split over the ranks')
   args = ap.parse_args()
   if args.warmup < 3 and args.impl == 'ours':

@@ -1,4 +1,4 @@
-/* rigl_b200 -- C ABI of the B200-native RigL hot path.
+/* rigl_b200 -- C ABI of the H100-native (sm_90a) RigL hot path.
  *
  * The reference (google-research/rigl) is pure Python/TensorFlow and has no FFI
  * of its own; these entry points are what a binding for its two hot paths
@@ -203,7 +203,7 @@ RIGL_API int rigl_sgd_plan_destroy(rigl_sgd_plan* plan);
 RIGL_API int rigl_sgd_plan_run(rigl_sgd_plan* plan, const float* lr_dev, float momentum, int nesterov, void* stream);
 
 /* ------------------------------------------------------------------------
- * Masked conv2d / linear as implicit GEMM (tcgen05 on sm_100a; a CUDA-core
+ * Masked conv2d / linear as implicit GEMM (wgmma on sm_90a; a CUDA-core
  * kernel serves shapes whose row pitch is not a 16-byte multiple).
  * Replaces layers.masked_conv2d / masked_fully_connected fprop and its two
  * gradient GEMMs (pruning_layers.py:72-172, 175-248; sparse_optimizers_base.py:
@@ -275,7 +275,7 @@ RIGL_API int rigl_stem_s2d_wgrad(const rigl_conv_desc* d, const void* xs, const 
 /* Small-Cin convs (cin <= 8, ksize <= 8: the 7x7x3 stem, resnet_model.py:620-633) WITHOUT a
  * patch matrix: the input is copied once into a zero-bordered 8-channel buffer `xp`
  * (rigl_smallc_padded_bytes); window tensor maps with a W stride of `stride` pixels then feed
- * the same tcgen05 kernels with ksize "taps" of K = 64 = 8 pixels x 8 channels.  `packed` here
+ * the same tensor-core kernels with ksize "taps" of K = 64 = 8 pixels x 8 channels.  `packed` here
  * is the stem-specific operand written by rigl_smallc_pack_weights from the SAME HWIO weights
  * and mask.  dw is the dense HWIO gradient as in rigl_conv2d_wgrad_dense. */
 RIGL_API int rigl_smallc_supported(const rigl_conv_desc* d);

@@ -75,11 +75,11 @@ class _CpuNet(object):
     self.bn, self.bn_order, self.p = {}, [], {}
     self.bn_init = None          # optional callable(key, channels) -> (gamma, beta) numpy
     self.trace = None            # optional list: receives (key, BN output) in execution order (debugging)
-    # bf16_activations: every activation tensor the B200 path stores (conv outputs, BN / ReLU / residual outputs,
+    # bf16_activations: every activation tensor the GPU path stores (conv outputs, BN / ReLU / residual outputs,
     # pooled features) and its gradient are rounded to bf16 at the same points; arithmetic inside an op stays fp32.
     # This is the bf16 configuration BASELINE.json names; False = the reference's fp32 CPU path (the timing port).
     # A 50-layer batch-normalised network at initialisation amplifies ANY perturbation by ~1.2x per layer
-    # (profiles/r02_whole_step_noise_growth.md), so only an oracle that rounds where the device rounds can be
+    # (tools/noise_growth.py), so only an oracle that rounds where the device rounds can be
     # compared layer by layer with it.
     self.bf16_act = False
 

@@ -323,7 +323,7 @@ def set_mask_update(mask, weights, random_grow_scores, drop_fraction, noise=None
 
 # --------------------------------------------------------------------------
 # rigl/sparse_optimizers.py -- the remaining optimizers on the same select primitive
-# (SURVEY 8(f) row 2: oracle first; the B200 product path for them is round-2 work)
+# (SURVEY 8(f) row 2: the oracle of the GPU product path for them)
 # --------------------------------------------------------------------------
 def momentum_ema_update(ema, masked_grad, momentum):
   """SparseMomentumOptimizer._before_apply_gradients (sparse_optimizers.py:172,195-197):

@@ -1,4 +1,4 @@
-"""In-tree build of librigl_b200.so (nvcc, sm_100a only).
+"""In-tree build of librigl_b200.so (nvcc, sm_90a only).
 
   python -m rigl_b200.build [--force] [--verbose]
 
@@ -19,7 +19,7 @@ LIB = os.path.join(HERE, 'librigl_b200.so')
 STAMP = os.path.join(HERE, 'build', 'stamp.txt')
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-std=c++17', '-lineinfo',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-lineinfo',
     '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '--expt-relaxed-constexpr',
     '-cudart', 'static',
 ]

@@ -13,7 +13,7 @@
 // Every kernel moves 16-byte vectors (8 channels) per thread with the channel dimension
 // innermost, so global traffic is fully coalesced; reductions go registers -> smem ->
 // per-block partials -> a tiny finalize kernel (fixed order: deterministic).
-// Tensors that fit in L2 take the single-launch variants (k_bn_fwd_fused / k_bn_bwd_fused: the
+// Tensors up to 64 MB take the single-launch variants (k_bn_fwd_fused / k_bn_bwd_fused: the
 // same three phases behind two grid barriers); rigl_bn_backward2 also sums the two gradients of a
 // forked block output inside the reduce pass.
 #include <cuda_bf16.h>
@@ -336,11 +336,14 @@ k_bn_bwd_apply(const __nv_bfloat16* __restrict__ g_or_da, const __nv_bfloat16* _
 
 
 // ----------------------------------------------------------------------------
-// Single-launch variants for tensors that fit in L2 (most ResNet-50 layers: 40 of its 53 BNs
+// Single-launch variants for tensors up to g_bn_fused_max_bytes (64 MB: 40 of ResNet-50's 53 BNs at batch 256
 // move <= 51 MB).  The three passes of a direction (column sums -> finalize -> apply) become
 // three phases of ONE persistent kernel separated by grid barriers: two dependent launch
 // boundaries (tail + ramp of every kernel, ~10 us of a ~35 us layer) disappear and the second pass
-// re-reads the rows this CTA just summed while they are still in L2.  Same arithmetic, same
+// re-reads the rows this CTA just summed, from L2 where they still fit.  The 64 MB cutoff was chosen on a chip
+// with a larger L2; on H100 (50 MB of L2) the 51 MB tensors re-read part of their rows from HBM, and the cutoff
+// has not been re-measured there (tools/bench_bn_layer.py compares the two paths per size; RIGL_BN_FUSED=0
+// selects the three-kernel path).  Same arithmetic, same
 // summation order (per-CTA partials in CTA order): results are bit-identical to the 3-kernel path
 // run with the same grid.  All CTAs must be co-resident (grid <= occupancy x SMs, checked by the host).
 // ----------------------------------------------------------------------------
@@ -609,8 +612,9 @@ static int fused_plan(int which, long long rows, int C, long long* rows_per_bloc
     env_read = true;
   }
   if (!g_bn_fused || C % 8 || C > 4096 || (size_t)rows * C * 2 > g_bn_fused_max_bytes) return 0;
-  // (measured on B200, tools/bench_bn_layer.py: the backward wins at every size <= 64 MB, the forward only
-  //  for wide layers -- with few vectors per row the 148 x 512-thread grid hides less latency than 3 big grids)
+  // (tools/bench_bn_layer.py compares the two: the backward wins at every size <= 64 MB, the forward only
+  //  for wide layers -- with few vectors per row the one-block-per-SM 512-thread grid hides less latency than 3
+  //  big grids)
   if (which == 0 && C < 512) return 0;
   const size_t smem = fused_smem(C);
   if (smem > 32 * 1024) return 0;
@@ -648,7 +652,7 @@ static int colsum_blocks(long long rows, int C, long long* rows_per_block) {
   const int V = C >> 3;
   const int vl = V < kBnThreads ? V : kBnThreads;
   const int rpi = kBnThreads / vl;
-  long long target = 148 * 6;                         // ~6 resident blocks per SM
+  long long target = kNumSmsHint * 6;                         // ~6 resident blocks per SM
   long long rpb = (rows + target - 1) / target;
   rpb = (rpb + rpi - 1) / rpi * rpi;
   if (rpb < rpi) rpb = rpi;
@@ -715,7 +719,7 @@ extern "C" int rigl_bn_forward_train(const void* y, const void* residual, const 
   RIGL_LAUNCH_CHECK("k_bn_finalize_fwd");
   const long long nvec = rows * (channels / 8);
   long long blocks = (nvec + kBnThreads - 1) / kBnThreads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSmsHint * 16) blocks = kNumSmsHint * 16;
   k_bn_apply<<<(unsigned)blocks, kBnThreads, 0, s>>>((const __nv_bfloat16*)y, (const __nv_bfloat16*)residual,
                                                      save_scale, save_shift, relu, nvec, channels / 8,
                                                      (__nv_bfloat16*)out, static_cast<uint8_t*>(relu_bits));
@@ -742,7 +746,7 @@ extern "C" int rigl_bn_forward_train_partials(const void* y, const void* residua
   RIGL_LAUNCH_CHECK("k_bn_finalize_fwd");
   const long long nvec = rows * (channels / 8);
   long long blocks = (nvec + kBnThreads - 1) / kBnThreads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSmsHint * 16) blocks = kNumSmsHint * 16;
   k_bn_apply<<<(unsigned)blocks, kBnThreads, 0, s>>>((const __nv_bfloat16*)y, (const __nv_bfloat16*)residual,
                                                      save_scale, save_shift, relu, nvec, channels / 8,
                                                      (__nv_bfloat16*)out, static_cast<uint8_t*>(relu_bits));
@@ -756,7 +760,7 @@ extern "C" int rigl_bn_apply(const void* y, const void* residual, const float* s
                "rigl_bn_apply: bad arguments");
   const long long nvec = rows * (channels / 8);
   long long blocks = (nvec + kBnThreads - 1) / kBnThreads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSmsHint * 16) blocks = kNumSmsHint * 16;
   k_bn_apply<<<(unsigned)blocks, kBnThreads, 0, (cudaStream_t)stream_>>>(
       (const __nv_bfloat16*)y, (const __nv_bfloat16*)residual, scale, shift, relu, nvec, channels / 8,
       (__nv_bfloat16*)out, nullptr);
@@ -835,7 +839,7 @@ extern "C" int rigl_bn_backward2(const void* da, const void* da2, const void* y,
   RIGL_LAUNCH_CHECK("k_bn_finalize_bwd");
   const long long nvec = rows * (channels / 8);
   long long blocks = (nvec + kBnThreads - 1) / kBnThreads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSmsHint * 16) blocks = kNumSmsHint * 16;
   k_bn_bwd_apply<<<(unsigned)blocks, kBnThreads, 0, s>>>(
       (const __nv_bfloat16*)(residual_form ? dresidual : da), (const __nv_bfloat16*)y, save_scale, save_shift, coef,
       (!residual_form && relu) ? 1 : 0, nvec, channels / 8, channels, (__nv_bfloat16*)dy);

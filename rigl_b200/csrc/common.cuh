@@ -1,4 +1,4 @@
-// Shared helpers for the rigl_b200 C-ABI library (sm_100a only).
+// Shared helpers for the rigl_b200 C-ABI library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,6 +9,10 @@
 #include "../../include/rigl_b200.h"
 
 namespace rigl {
+
+// SM count of an H100 SXM: sizes grids before (or without) a device query.  Grid-size heuristics only; the
+// persistent tensor-core kernels size their grids from the device's own count.
+constexpr int kNumSmsHint = 132;
 
 void set_error(const char* fmt, ...);
 extern std::atomic<uint64_t> g_launches;

@@ -1,5 +1,5 @@
 // C-ABI entry points of the masked conv / linear path: argument validation and
-// the shape dispatch between the tcgen05 implicit-GEMM kernels (igemm_tc.cu)
+// the shape dispatch between the wgmma implicit-GEMM kernels (igemm_tc.cu)
 // and the CUDA-core kernels (conv_simt.cu).
 #include <stdlib.h>
 

@@ -51,7 +51,7 @@ int simt_dgrad(const ConvGeom& g, const void* dy, const void* w_fprop, void* dx,
 int simt_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float beta, cudaStream_t s);
 int simt_im2col(const ConvGeom& g, const void* x, void* out, int64_t out_pitch, cudaStream_t s);
 
-// tcgen05 path (igemm_tc.cu)
+// tensor-core path (igemm_tc.cu)
 bool tc_supported(const ConvGeom& g, int which /*0 fprop, 1 dgrad, 2 wgrad*/);
 size_t tc_workspace_bytes(const ConvGeom& g);
 int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32,

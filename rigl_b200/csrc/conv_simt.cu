@@ -1,9 +1,9 @@
 // CUDA-core (SIMT) masked conv / linear kernels: the shape-agnostic path.
 //
-// Used (a) for shapes the TMA/tcgen05 path cannot address (channel counts that
+// Used (a) for shapes the TMA/wgmma path cannot address (channel counts that
 // are not multiples of 8, i.e. row pitches that are not 16-byte multiples: the
 // 7x7x3 stem, 10-way logits, unit-test layers) and (b) as the on-device
-// cross-check of the tcgen05 kernels (RIGL_FORCE_SIMT=1).  bf16 operands, fp32
+// cross-check of the wgmma kernels (RIGL_FORCE_SIMT=1).  bf16 operands, fp32
 // accumulation, same packed masked-weight operands as the tensor-core path.
 #include <cuda_bf16.h>
 

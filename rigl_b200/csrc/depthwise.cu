@@ -3,9 +3,8 @@
 //
 // Replaces depthwise_conv2d_fixed_padding of the reference's MobileNet-v1
 // (rigl/imagenet_resnet/mobilenetv1_model.py:120-153, called from mbv1_block_ :186-196).  The depthwise convs are
-// NOT masked in the reference (only the pointwise 1x1 convs and the classifier are), but they are a third of the
-// C4 step on the stock cuDNN kernels (profiles/r02_step_launches_c4_mobilenet.md: 4.8 of 15 ms, the data gradient
-// alone 2.5 ms for 2 GB of traffic), so SURVEY 8(f) row 4 ("depthwise") is built as three streaming kernels.
+// NOT masked in the reference (only the pointwise 1x1 convs and the classifier are), but they are a large share of
+// the C4 step on the stock cuDNN kernels, so SURVEY 8(f) row 4 ("depthwise") is built as three streaming kernels.
 //
 // One thread = 8 channels (one 16-byte vector), channels innermost.  Weights: fp32 master [C][1][3][3] (the torch /
 // TF depthwise layout flattened as c*9 + kh*3 + kw), rounded to bf16 on load like the activations' compute type;
@@ -226,7 +225,7 @@ static int dw_wgrad_blocks(const DwGeom& g, long long* rows_per_block) {
   const long long rows = (long long)g.n * g.oh;
   const int V = g.c / 8, bx = V < 32 ? V : 32;
   const int groups = (V + bx - 1) / bx;
-  long long target = (148 * 4 + groups - 1) / groups;          // ~4 CTAs per SM in total
+  long long target = (kNumSmsHint * 4 + groups - 1) / groups;          // ~4 CTAs per SM in total
   if (target > rows) target = rows;
   if (target < 1) target = 1;
   *rows_per_block = (rows + target - 1) / target;

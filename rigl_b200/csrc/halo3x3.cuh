@@ -2,17 +2,18 @@
 //
 // The generic implicit-GEMM kernels fetch one shifted TMA box per filter tap, so a 3x3 layer
 // reads its input NINE times from L2; at 64 channels there is so little math per byte that the
-// chip-wide L2 -> SM bandwidth (~6300 B/clk) is what bounds them (200 us for 59 GFLOP).
+// chip-wide L2 -> SM bandwidth is what bounds them.
 // Here a CTA loads ONE halo tile -- (R+2) image rows, each padded to a power-of-two pitch Wp
-// >= W+2 by TMA out-of-bounds zero fill -- and feeds all nine taps from it: the UMMA shared
-// memory descriptor of tap (dh, dw) simply starts (dh+1)*Wp + (dw+1) rows (128 B each) further
-// down the tile.  SWIZZLE_128B is a function of the absolute shared-memory address, so a start
-// address that is not 1024-byte aligned addresses the same swizzled bytes TMA wrote (verified on
-// B200 by tools/umma_shift_probe.cu for every row shift, K-major and MN-major).
+// >= W+2 by TMA out-of-bounds zero fill -- and feeds all nine taps from it: the A operand of tap
+// (dh, dw) simply starts (dh+1)*Wp + (dw+1) rows (128 B each) further down the tile.  Such a start
+// is not aligned to the 1024-byte swizzle period, so the A fragments are loaded with ldmatrix at
+// explicitly swizzled addresses (the TMA writes SWIZZLE_128B as a function of the absolute
+// shared-memory address) and fed to the register-A form of wgmma; the B operands (resident
+// weights, the dY tile) stay on aligned shared-memory descriptors.
 //
 //   position q = r*Wp + c   (r = row inside the strip, c = column, c >= W is padding)
 //   fprop/dgrad: D[q, n]   = sum_tap sum_k  X[q + off(tap), k] * Wt[tap][n, k]     (K-major A)
-//   wgrad:       D[tap][ci, co] = sum_q X[q + off(tap), ci] * dY[q, co]            (MN-major A, B)
+//   wgrad:       D[tap][ci, co] = sum_q X[q + off(tap), ci] * dY[q, co]            (A = X^T via ldmatrix.trans)
 // Padding columns of the OUTPUT are clipped by the TMA store (fprop/dgrad) or multiply dY zeros
 // (wgrad: the dY tile is loaded with the same pitch, its padding columns zero-filled).
 //
@@ -37,16 +38,26 @@ struct HaloParams {
 
 constexpr uint32_t kHaloBTapBytes = 64 * 64 * 2;        // one tap of the resident weight tile: 8 KB
 constexpr uint32_t kHaloSlabBytes = 128 * 64 * 2;       // output staging slab: 16 KB
+// wgrad: three consumer warpgroups, one per filter row, and no separate producer warpgroup (thread 0 issues the
+// loads): at 384 threads a thread may hold 168 registers, room for the 96 accumulator registers of a filter row
+// plus two steps of A fragments in flight without spilling or serialising the wgmma stream.
+constexpr int kHaloWgradThreads = 384;
+
+// The register-A fragments of an in-flight wgmma must keep their registers until the MMA has read them:
+// `keep_frag` after the wait that retires the MMA keeps the values (and so their registers) live up to it.
+__device__ __forceinline__ void keep_frag(const uint32_t (&a)[4]) {
+  asm volatile("" ::"r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]) : "memory");
+}
 
 // ----------------------------------------------------------------------------
 // fprop / dgrad: weights of this CTA's 64-channel N tile stay resident in shared memory.
-// grid = (CTAs over strips, N tiles).  warp 0: TMA, warp 1: MMA, warps 2-5: epilogue.
+// grid = (CTAs over strips, N tiles).  warp 0: TMA; warpgroups 1-2: MMA + epilogue, 64 positions of each
+// 128-position M tile each.
 // ----------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads, 1)
 k_halo3x3_kmajor(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
                  const __grid_constant__ CUtensorMap omap, const HaloParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr uint32_t kIdesc = make_idesc_bf16(128, 64, 0, 0);
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t b_base = smem_base;                                   // 9 taps x 8 KB
   const uint32_t a_base = b_base + 9 * kHaloBTapBytes;                 // nbuf halo tiles
@@ -55,25 +66,16 @@ k_halo3x3_kmajor(const __grid_constant__ CUtensorMap amap, const __grid_constant
   const uint32_t b_full = bar_base;
   auto a_full = [&](int b) { return bar_base + 8u * (1 + b); };
   auto a_empty = [&](int b) { return bar_base + 8u * (5 + b); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (9 + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (11 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * 13;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tile = blockIdx.y;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&amap); prefetch_tmap(&bmap); prefetch_tmap(&omap);
     mbar_init(b_full, 1);
-    for (int b = 0; b < p.nbuf; ++b) { mbar_init(a_full(b), 1); mbar_init(a_empty(b), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
+    for (int b = 0; b < p.nbuf; ++b) { mbar_init(a_full(b), 1); mbar_init(a_empty(b), kConsumerWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   const int rt = 128 / p.Wp;                              // image rows per M tile
 
   if (warp == 0) {
@@ -89,222 +91,173 @@ k_halo3x3_kmajor(const __grid_constant__ CUtensorMap amap, const __grid_constant
         if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    // The whole warp runs the loop converged; one elected lane issues (see ptx::elect_one).
+  } else if (warp >= kConsumerWarp0) {
+    const int cw = warp - kConsumerWarp0;
+    const int wg = cw >> 2;
+    const int row = 64 * wg + 16 * (cw & 3) + (lane >> 2);             // accumulator rows row, row + 8
+    // ldmatrix: lane supplies position lrow of matrix lane / 8 (rows +8 for matrices 1 and 3, K +8 for 2 and 3)
+    const int lrow = 64 * wg + 16 * (cw & 3) + (lane & 7) + 8 * ((lane >> 3) & 1);
+    const uint32_t lk = (uint32_t)(lane >> 4) * 16u;
+    const bool issuer = (cw == 0 && lane == 0);
+    const uint64_t b_desc0 = make_smem_desc(b_base, 16, 1024);
     mbar_wait(b_full, 0);
     int buf = 0; uint32_t phase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
-    const uint64_t b_desc0 = make_smem_desc(b_base, 16, 1024);
-    for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
-      mbar_wait(a_full(buf), phase);
-      tc_fence_after();
-      const uint64_t a_desc0 = make_smem_desc(a_base + buf * p.a_buf_bytes, 16, 1024);
-      for (int t = 0; t < p.T; ++t) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 64);
-        if (elect_one()) {
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {              // descriptor start addresses are in 16-byte units
-            const uint64_t da = a_desc0 + (uint64_t)((t * 128 + p.row_off[tap]) * 8);
-            const uint64_t db = b_desc0 + (uint64_t)(tap * (kHaloBTapBytes >> 4));
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, da + 2 * k, db + 2 * k, kIdesc, (tap == 0 && k == 0) ? 0u : 1u);
-          }
-          umma_commit(tfull_bar(acc));
-        }
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-      if (elect_one()) umma_commit(a_empty(buf));          // halo tile reusable once its MMAs retire
-      __syncwarp();
-      if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
-    }
-  } else {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;                      // position inside the M tile
-    const bool issuer = (warp == 2 && lane == 0);
-    int acc = 0; uint32_t acc_phase = 0;
     uint32_t slab_ctr = 0;
     for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
       const int n = strip / p.strips_per_image, h0 = (strip % p.strips_per_image) * p.R;
+      mbar_wait(a_full(buf), phase);
+      const uint32_t a_tile = a_base + buf * p.a_buf_bytes;
       for (int t = 0; t < p.T; ++t) {
-        mbar_wait(tfull_bar(acc), acc_phase);
-        tc_fence_after();
+        float acc[32];
+        zero_acc(acc);
+        uint32_t a[2][4][4];
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t src = a_tile + (uint32_t)(t * 128 + lrow + p.row_off[tap]) * 128u + lk;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) ldmatrix_x4(a[tap & 1][k], swz128(src + 32u * k));
+          fence_regs(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k)                     // descriptor start addresses are in 16-byte units
+            Wgmma<64>::rs<0>(acc, a[tap & 1][k], b_desc0 + (uint64_t)(tap * (kHaloBTapBytes >> 4) + 2 * k));
+          wgmma_commit();
+          wgmma_wait<1>();                                // the previous tap's fragments may be overwritten
+          if (tap > 0) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) keep_frag(a[(tap + 1) & 1][k]);
+          }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) keep_frag(a[0][k]);
         const uint32_t slab = out_base + (slab_ctr & 1u) * kHaloSlabBytes;
         if (issuer) tma_store_wait_read<1>();
-        named_bar_sync(1, 128);
-        uint32_t r0[32], r1[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * 64), r0);
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * 64 + 32), r1);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(acc));       // accumulator drained into registers
-        const uint32_t row_addr = slab + (uint32_t)row * 128u;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          uint32_t pk[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int e = 8 * j + 2 * q;
-            const float a = __uint_as_float(e < 32 ? r0[e] : r1[e - 32]);
-            const float b = __uint_as_float(e + 1 < 32 ? r0[e + 1] : r1[e + 1 - 32]);
-            __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-            pk[q] = *reinterpret_cast<uint32_t*>(&h);
-          }
-          const uint32_t dst = row_addr + (uint32_t)((j ^ (row & 7)) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]),
-                       "r"(pk[3])
-                       : "memory");
-        }
+        named_bar_sync(1, kConsumerThreads);
+        stage_slab<0>(acc, slab, row, true, true, lane);  // columns >= W and rows >= H are clipped by the store
         fence_proxy_async_smem();
-        named_bar_sync(1, 128);
-        if (issuer) {                                      // columns >= W and rows >= H are clipped by TMA
+        named_bar_sync(1, kConsumerThreads);
+        if (issuer) {
           tma_store_4d(&omap, slab, n_tile * 64, 0, h0 + t * rt, n);
           tma_store_commit();
         }
         ++slab_ctr;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(a_empty(buf));           // every MMA of this warp that read the tile has retired
+      if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
     }
     if (issuer) tma_store_wait_all();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
   }
 }
 
 // ----------------------------------------------------------------------------
-// wgrad: every CTA accumulates all nine taps over its strips in TMEM (five 128 x 64
-// accumulators: two taps per MMA, the taps being the two 64-channel M atoms of an MN-major A
-// operand whose atom stride (LBO) is the distance between the taps' halo rows), then writes one
-// fp32 partial [9][ci][co]; k_splitk_reduce sums the partials in CTA order (deterministic).
+// wgrad: every CTA accumulates all nine taps over its strips in registers -- consumer warpgroup kh holds the three 64 x 64 accumulators of filter row kh -- then writes one fp32 partial [9][ci][co]; k_splitk_reduce
+// sums the partials in CTA order (deterministic).
 // ----------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kHaloWgradThreads, 1)
 k_halo3x3_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap dymap,
                 const HaloParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr uint32_t kIdesc = make_idesc_bf16(128, 64, 1, 1);
+  constexpr int kWarps = 12;                                           // consumer warps
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t dy_bytes = (uint32_t)(p.R * p.Wp) * 128u;
   const uint32_t stage_bytes = p.a_buf_bytes + dy_bytes;               // [x halo | dy]
   const uint32_t bar_base = smem_base + p.nbuf * stage_bytes;
   auto full_bar = [&](int b) { return bar_base + 8u * b; };
   auto empty_bar = [&](int b) { return bar_base + 8u * (4 + b); };
-  const uint32_t tfull = bar_base + 8u * 8;
-  const uint32_t tmem_slot = bar_base + 8u * 9;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&xmap); prefetch_tmap(&dymap);
-    for (int b = 0; b < p.nbuf; ++b) { mbar_init(full_bar(b), 1); mbar_init(empty_bar(b), 1); }
-    mbar_init(tfull, 1);
+    for (int b = 0; b < p.nbuf; ++b) { mbar_init(full_bar(b), 1); mbar_init(empty_bar(b), kWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
   // The slack rows behind each halo tile are read (against zero dY columns): they must be finite.
   {
     const uint32_t halo_rows_bytes = p.a_tx_bytes;
     const uint32_t slack = p.a_buf_bytes - halo_rows_bytes;
     for (int b = 0; b < p.nbuf; ++b)
-      for (uint32_t i = threadIdx.x * 16u; i < slack; i += kThreads * 16u)
+      for (uint32_t i = threadIdx.x * 16u; i < slack; i += kHaloWgradThreads * 16u)
         asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(smem_base + b * stage_bytes + halo_rows_bytes + i), "r"(0u)
                      : "memory");
     fence_proxy_async_smem();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int buf = 0; uint32_t phase = 0;
-      for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
-        const int n = strip / p.strips_per_image, h0 = (strip % p.strips_per_image) * p.R;
-        mbar_wait(empty_bar(buf), phase ^ 1u);
-        mbar_arrive_expect_tx(full_bar(buf), p.a_tx_bytes + dy_bytes);
-        const uint32_t x_dst = smem_base + buf * stage_bytes;
-        tma_load_4d(x_dst, &xmap, full_bar(buf), 0, -1, h0 - 1, n);
-        tma_load_4d(x_dst + p.a_buf_bytes, &dymap, full_bar(buf), 0, 0, h0, n);
-        if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp == 1) {
-    int buf = 0; uint32_t phase = 0;                       // converged warp, one elected lane issues
-    bool first = true;
+  auto issue = [&](int strip, int b) {                     // (thread 0) halo tile + dY tile of `strip` into buffer b
+    const int n = strip / p.strips_per_image, h0 = (strip % p.strips_per_image) * p.R;
+    mbar_arrive_expect_tx(full_bar(b), p.a_tx_bytes + dy_bytes);
+    const uint32_t x_dst = smem_base + b * stage_bytes;
+    tma_load_4d(x_dst, &xmap, full_bar(b), 0, -1, h0 - 1, n);
+    tma_load_4d(x_dst + p.a_buf_bytes, &dymap, full_bar(b), 0, 0, h0, n);
+  };
+  if (threadIdx.x == 0) {                                  // fill every buffer once
+    int strip = blockIdx.x;
+    for (int b = 0; b < p.nbuf && strip < p.total_strips; ++b, strip += gridDim.x) issue(strip, b);
+  }
+  {
+    const int cw = warp;                                   // 0..11
+    const int kh = cw >> 2, wq = cw & 3;                   // filter row; 16 input channels 16wq..16wq+15
+    // ldmatrix.trans: lane supplies position (K) row 8 * (lane >> 4) + (lane & 7) of matrix lane / 8, whose 8
+    // channels are chunk 2wq + ((lane >> 3) & 1) of the 128-byte row.
+    const uint32_t lpos = (uint32_t)(8 * (lane >> 4) + (lane & 7));
+    const uint32_t lchunk = (uint32_t)(2 * wq + ((lane >> 3) & 1)) * 16u;
+    float acc[3][32];
+#pragma unroll
+    for (int kw = 0; kw < 3; ++kw) zero_acc(acc[kw]);
+    uint32_t a[3][4];
+    int buf = 0; uint32_t phase = 0;
     const int ksteps = p.R * p.Wp / 16;
     for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
       mbar_wait(full_bar(buf), phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t x_src = smem_base + buf * stage_bytes;
-        const uint64_t db0 = make_smem_desc(x_src + p.a_buf_bytes, 8192, 1024);
-        uint64_t da0[5];
-#pragma unroll
-        for (int j = 0; j < 5; ++j) {
-          // accumulator j holds taps (2j, 2j+1); the last one pairs (7, 8): tap 7 is computed twice
-          const int t0 = j < 4 ? 2 * j : 7, t1 = t0 + 1;
-          da0[j] = make_smem_desc(x_src + (uint32_t)p.row_off[t0] * 128u,
-                                  (uint32_t)(p.row_off[t1] - p.row_off[t0]) * 128u, 1024);
-        }
+      const uint32_t x_src = smem_base + buf * stage_bytes;
+      const uint64_t db0 = make_smem_desc(x_src + p.a_buf_bytes, 8192, 1024);
+      const uint32_t a0 = x_src + (uint32_t)(kh * p.Wp + (int)lpos) * 128u + lchunk;   // row_off[3kh] = kh * Wp
 #pragma unroll 2
-        for (int k = 0; k < ksteps; ++k) {                 // 16 positions = +128 in the 16-byte address field
+      for (int k = 0; k < ksteps; ++k) {                   // 16 positions = +2048 B of x and of dY rows
+        // the three taps of filter row kh as one wgmma group; its fragments are reloaded only after it retires
 #pragma unroll
-          for (int j = 0; j < 5; ++j)
-            umma_bf16(tmem_base + (uint32_t)(j * 64), da0[j] + (uint64_t)(128 * k), db0 + (uint64_t)(128 * k), kIdesc,
-                      (first && k == 0) ? 0u : 1u);
+        for (int kw = 0; kw < 3; ++kw) ldmatrix_x4_trans(a[kw], swz128(a0 + (uint32_t)(16 * k + kw) * 128u));
+        wgmma_fence();
+#pragma unroll
+        for (int kw = 0; kw < 3; ++kw) Wgmma<64>::rs<1>(acc[kw], a[kw], db0 + (uint64_t)(128 * k));
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int kw = 0; kw < 3; ++kw) keep_frag(a[kw]);
+      }
+#pragma unroll
+      for (int kw = 0; kw < 3; ++kw) fence_regs(acc[kw]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(buf));
+      if (threadIdx.x == 0) {                              // refill this buffer once all 12 warps have released it
+        const int next = strip + p.nbuf * (int)gridDim.x;
+        if (next < p.total_strips) {
+          mbar_wait(empty_bar(buf), phase);
+          issue(next, buf);
         }
-        umma_commit(empty_bar(buf));
       }
       __syncwarp();
-      first = false;
       if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
     }
-    if (elect_one()) umma_commit(tfull);
-    __syncwarp();
-  } else {
-    const int quad = warp & 3;
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-    const int ci = (quad & 1) * 32 + lane;
     float* part = p.wgrad_out + (size_t)blockIdx.x * 9 * p.ci * p.N;
-#pragma unroll 1
-    for (int j = 0; j < 5; ++j) {
-      const int t0 = j < 4 ? 2 * j : 7;
-      const int tap = t0 + (quad >> 1);
-      const bool dup = (j == 4 && (quad >> 1) == 0);       // second copy of tap 7
-      float* dst_row = part + ((size_t)tap * p.ci + ci) * p.N;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t r32[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(j * 64 + c0), r32);
-        tmem_ld_wait();
-        if (!dup && ci < p.ci && c0 < p.N) {
 #pragma unroll
-          for (int q = 0; q < 32; q += 4) {
-            if (c0 + q + 4 <= p.N) {
-              *reinterpret_cast<float4*>(dst_row + c0 + q) =
-                  make_float4(__uint_as_float(r32[q]), __uint_as_float(r32[q + 1]), __uint_as_float(r32[q + 2]),
-                              __uint_as_float(r32[q + 3]));
-            } else {
-              for (int t = 0; t < 4 && c0 + q + t < p.N; ++t) dst_row[c0 + q + t] = __uint_as_float(r32[q + t]);
-            }
-          }
+    for (int kw = 0; kw < 3; ++kw) {
+      const int tap = 3 * kh + kw;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int ci = 16 * wq + (lane >> 2) + 8 * h;
+        if (ci >= p.ci) continue;
+        float* dst_row = part + ((size_t)tap * p.ci + ci) * p.N;
+#pragma unroll
+        for (int jc = 0; jc < 8; ++jc) {
+          const int co = 8 * jc + 2 * (lane & 3);                     // co is even and p.N % 8 == 0
+          if (co < p.N) *reinterpret_cast<float2*>(dst_row + co) = make_float2(acc[kw][4 * jc + 2 * h], acc[kw][4 * jc + 2 * h + 1]);
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -365,7 +318,7 @@ static bool halo_wgrad_ok(const ConvGeom& g, HaloParams* p) {
 }
 static int halo_wgrad_grid(const HaloParams& p) {
   ensure_driver();
-  const int sms = g_num_sms > 0 ? g_num_sms : 148;
+  const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   return p.total_strips < sms ? p.total_strips : sms;
 }
 static size_t halo_wgrad_ws_elems(const ConvGeom& g, const HaloParams& p) {
@@ -402,7 +355,7 @@ static int halo_launch_kmajor(HaloParams p, const void* in, int kred, int in_pit
     configured = smem;
   }
   const int n_tiles = (n_out + 63) / 64;
-  const int sms = g_num_sms > 0 ? g_num_sms : 148;
+  const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   int gx = sms / n_tiles;
   if (gx < 1) gx = 1;
   if (gx > p.total_strips) gx = p.total_strips;
@@ -431,7 +384,7 @@ static int halo_launch_wgrad(HaloParams p, const ConvGeom& g, const void* x, con
     RIGL_CUDA(cudaFuncSetAttribute(k_halo3x3_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = smem;
   }
-  k_halo3x3_wgrad<<<(unsigned)halo_wgrad_grid(p), kThreads, smem, s>>>(xmap, dymap, p);
+  k_halo3x3_wgrad<<<(unsigned)halo_wgrad_grid(p), kHaloWgradThreads, smem, s>>>(xmap, dymap, p);
   RIGL_LAUNCH_CHECK("k_halo3x3_wgrad");
   return RIGL_OK;
 }

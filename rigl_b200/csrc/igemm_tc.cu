@@ -1,4 +1,4 @@
-// Masked conv2d / linear as implicit GEMM on the 5th-gen tensor cores (sm_100a).
+// Masked conv2d / linear as implicit GEMM on the Hopper tensor cores (sm_90a, wgmma).
 //
 //   fprop : y[pix, co]  = sum_{tap, ci} x[pix (+) tap, ci] * Wm[tap][co][ci]
 //   dgrad : dx[pix, ci] = sum_{tap, co} dy[pix (-) tap, co] * Wm[tap][ci][co]
@@ -12,19 +12,16 @@
 // (cp.async.bulk.tensor.4d) whose out-of-bounds zero fill implements the padding.
 // Stride-2 convs read through four parity sub-grid tensor maps (same trick,
 // element strides doubled), so every conv shape in ResNet/WRN is a plain loop of
-// TMA boxes + tcgen05.mma with fp32 accumulators in TMEM.
+// TMA boxes + wgmma.mma_async with fp32 accumulators in registers.
 //
-// Kernel organisation (persistent, one CTA per SM, 192 threads):
-//   warp 0    : TMA producer (converged warp, one elect.sync lane issues)   smem ring, full/empty mbarriers
-//   warp 1    : TMEM allocator + MMA issuer (same pattern): tcgen05.mma kind::f16, M = 128 per CTA
-//   warps 2-5 : epilogue: tcgen05.ld 32x32b -> bf16 -> swizzled smem slab -> TMA store (or direct
-//               fp32/bias stores), double-buffered accumulators so the epilogue of tile i overlaps
-//               the main loop of tile i+1.
-// Variants: k_igemm_kmajor (one CTA per tile, optional 2-CTA weight multicast, optional fused BN
-// statistics), k_igemm_kmajor2 (default for fprop/dgrad: CTA pair, tcgen05 cta_group::2, M = 256),
-// k_igemm_wgrad, and -- textually included below -- halo3x3.cuh (3x3/s1 layers with <= 64 channels:
-// one smem halo tile feeds all nine taps) and stem_s2d.cuh (experimental).  Measured limits that
-// shape these kernels (TMA ingest 54 B/clk/SM, cycles per MMA by N): DESIGN.md 3.2 / 3.7.
+// Kernel organisation (persistent, one CTA per SM, 384 threads = three warpgroups):
+//   warp 0        : TMA producer (converged warp, one elected lane issues)   smem ring, full/empty mbarriers
+//   warpgroups 1-2: consumers: each issues the wgmma for 64 of the tile's 128 rows, then runs the epilogue of
+//                   those rows from its registers: bf16 -> swizzled smem slab -> TMA store (or direct fp32/bias
+//                   stores); the producer refills the ring for the next tile meanwhile.
+// Variants: k_igemm_kmajor (fprop/dgrad, optional fused BN statistics), k_igemm_wgrad, and -- textually included
+// below -- halo3x3.cuh (3x3/s1 layers with <= 64 channels: one smem halo tile feeds all nine taps) and
+// stem_s2d.cuh (the 7x7/2 stem).  DESIGN.md 3 describes the design.
 // fprop/dgrad use K-major operands; wgrad reduces over pixels, so both operands are
 // MN-major views of the NHWC tensors (no transposes are materialised) and the
 // pixel range is split across CTAs (deterministic two-pass split-K).
@@ -45,9 +42,12 @@ namespace rigl {
 using namespace ptx;
 
 constexpr int kMaxTaps = 9;
-constexpr int kBM = 128;            // UMMA M
+constexpr int kBM = 128;            // M tile: two warpgroups x 64 rows
 constexpr int kBK = 64;             // K block: 64 bf16 = one 128B swizzle row
-constexpr int kThreads = 192;
+constexpr int kThreads = 384;       // warpgroup 0: producer; warpgroups 1-2: consumers
+constexpr int kConsumerWarp0 = 4;
+constexpr int kConsumerWarps = 8;
+constexpr int kConsumerThreads = 256;
 
 struct TapInfo {
   int8_t map_id, dh, dw, pad;
@@ -71,7 +71,6 @@ struct IgemmParams {
   int nnz_tap_stride, nnz_n_stride, nnz_k_stride;
   int tma_store;                    // 1: epilogue stages bf16 tiles in smem and TMA-stores them
   float* bn_partial;                // optional [gridDim.x][2][N]: per-CTA column sums / sums of squares of D
-  int pair_local;                   // CTA-pair kernel: each CTA's TMA completes on its OWN barrier (see k_igemm_kmajor2)
   int stats_dbg;                    // development: 1 = statistics without the global REDs, 2 = without the smem pass
 };
 
@@ -92,15 +91,16 @@ __device__ __forceinline__ bool weight_block_live(const IgemmParams& p, int tap_
 
 
 // Liveness of every (tap, K block) of one N tile as a bitmask in shared memory, computed by a
-// whole warp at the start of a tile (one round of parallel loads) instead of by the issuing
-// thread once per K block: the single-thread TMA / MMA issue loops are instruction-latency bound
-// (about 900 clk per stage with the survivor-table loads inline, which hid the TMA and tensor
-// limits), so everything that can leave them does.  Block 0 is always live (it initialises D).
+// whole warp at the start of a tile (one round of parallel loads) instead of once per K block
+// inside the issue loops, which are instruction-latency bound.  Block 0 is always live.
 constexpr int kLiveWords = 10;        // 320 (tap, K block) pairs; longer reductions run without skipping
+__device__ __forceinline__ bool live_mask_used(const IgemmParams& p) {   // no table (or too long): everything is live
+  return p.nnz != nullptr && p.ntaps * p.kblks <= kLiveWords * 32;
+}
 template <int kBN64>
 __device__ __forceinline__ bool build_live_mask(const IgemmParams& p, int n_tile, int lane, uint32_t* mask_smem) {
   const int nkb = p.ntaps * p.kblks;
-  if (p.nnz == nullptr || nkb > kLiveWords * 32) return false;       // no table (or too long): everything is live
+  if (!live_mask_used(p)) return false;
   for (int w = 0; w * 32 < nkb; ++w) {
     const int j = w * 32 + lane;
     bool live = true;
@@ -123,7 +123,7 @@ __device__ __forceinline__ bool build_live_mask(const IgemmParams& p, int n_tile
 //   swizzle phases, so the 32 lanes of every LDS.32 hit 32 different banks.
 // 32 LDS + ~130 FP ops per thread per slab, two shuffles per statistic, and ONE RED per (slab, channel, statistic):
 // each table entry is only ever touched by one lane of one warp, in tile order, so the fp32 sums are deterministic.
-// Rows outside the pixel grid are written as zeros by their owner (see the staging loops), so they do not count.
+// Rows outside the pixel grid are written as zeros by their owner (see stage_slab), so they do not count.
 __device__ __forceinline__ void slab_bn_stats(uint32_t slab, int quad, int lane, float* __restrict__ bn_row, int co0,
                                               int n, int dbg) {
   const int cp = lane & 7, g = lane >> 3;
@@ -152,11 +152,55 @@ __device__ __forceinline__ void slab_bn_stats(uint32_t slab, int quad, int lane,
   }
 }
 
-// CL = CTAs per cluster (1 or 2).  With CL == 2 the two CTAs work on the two M tiles of a tile
-// PAIR that share the weight tile: each loads HALF of B and multicasts it into both CTAs'
-// shared memory, which cuts the L2->smem bytes per FLOP by a third (these kernels are bound
-// by that traffic, not by the tensor pipe).  A stage is recycled only when BOTH consumers
-// have released it (empty barriers count CL arrivals; tcgen05.commit multicasts them).
+// Accumulator fragment of a warpgroup's m64nN wgmma: register 4*j + 2*h + e holds
+//   row 16 * (warp % 4) + lane / 4 + 8 * h,  column 8 * j + 2 * (lane % 4) + e.
+// stage_slab writes columns [64 * S, 64 * S + 64) of this thread's two rows (tile rows `row` and `row + 8`) as bf16
+// into a 128-row staging slab (128-byte rows, 16-byte chunks XOR-swizzled by row & 7, the TMA store's layout).
+// Rows outside the output grid are written as zeros (they are clipped by the store but read by the statistics).
+template <int S, int R>
+__device__ __forceinline__ void stage_slab(const float (&d)[R], uint32_t slab, int row, bool ok0, bool ok1, int lane) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row + 8 * h;
+      const int e = 4 * (8 * S + jj) + 2 * h;
+      __nv_bfloat162 v = __floats2bfloat162_rn(d[e], d[e + 1]);
+      const uint32_t w = (h ? ok1 : ok0) ? *reinterpret_cast<uint32_t*>(&v) : 0u;
+      const uint32_t dst = slab + (uint32_t)r * 128u + (uint32_t)((jj ^ (r & 7)) << 4) + (uint32_t)(lane & 3) * 4u;
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(w) : "memory");
+    }
+  }
+}
+
+template <int R>
+__device__ __forceinline__ void zero_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) d[i] = 0.f;
+}
+
+// A consumer warp's release of a ring slot: with CL == 2 the slot of BOTH CTAs is filled by both producers (each
+// multicasts its half of the shared operand), so the release goes to the empty barrier of every CTA.
+template <int CL>
+__device__ __forceinline__ void release_stage(uint32_t bar) {
+  if (CL == 1) {
+    mbar_arrive(bar);
+  } else {
+#pragma unroll
+    for (int c = 0; c < CL; ++c) mbar_arrive_cluster(bar, (uint32_t)c);
+  }
+}
+
+// Warp roles (384 threads, one CTA per SM, persistent over tiles):
+//   warp 0       : TMA producer (converged warp, one elected lane issues)   smem ring, full/empty mbarriers
+//   warps 1-3    : idle
+//   warps 4-11   : two consumer warpgroups; warpgroup w issues the wgmma of pixel rows 64w..64w+63 of the tile
+//                  (A from shared memory, K-major), keeps its 64 x BN fp32 accumulators in registers, then runs
+//                  the epilogue for those rows: bf16 -> swizzled smem slab -> TMA store (or direct fp32/bias
+//                  stores).  The producer keeps filling the ring for the next tile meanwhile.
+// CL = CTAs per cluster (1 or 2).  With CL == 2 the two CTAs work on the two M tiles of a tile PAIR that share the
+// weight tile: each loads HALF of B and multicasts it into both CTAs' shared memory.  A stage is refilled only when
+// the consumers of BOTH CTAs have released it: every consumer warp arrives on the empty barrier of each CTA.
 template <int BN, int STAGES, int CL>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
@@ -165,254 +209,172 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
   constexpr uint32_t kABytes = kBM * kBK * 2;        // 16 KB
   constexpr uint32_t kBBytes = BN * kBK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  constexpr uint32_t kIdesc = make_idesc_bf16(kBM, BN, 0, 0);
-
   constexpr uint32_t kSlabBytes = kBM * 64 * 2;       // one 128-pixel x 64-channel output slab
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t out_base = smem_base + STAGES * kStageBytes;          // 2 staging slabs (1024B aligned)
   const uint32_t bar_base = out_base + 2 * kSlabBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
-  __shared__ uint32_t live_prod[kLiveWords], live_mma[kLiveWords];
+  // live_cons[warpgroup][tile parity]: one liveness mask per consumer warpgroup, double-buffered over tiles
+  __shared__ uint32_t live_prod[kLiveWords], live_cons[2][2][kLiveWords];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int i = 0; i < 4; ++i) prefetch_tmap(&amaps.a[i]);
     prefetch_tmap(&bmap);
     if (p.tma_store) prefetch_tmap(&omap);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CL); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps * CL); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
-  if (CL > 1) cluster_sync_all(); else __syncthreads();       // peers' barriers are live before any multicast
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  if (CL > 1) cluster_sync_all(); else __syncthreads();     // peers' barriers are live before any multicast
 
-  // Tile schedule: a "pair" = CL consecutive M tiles x one N tile; pairs are dealt round-robin to
-  // clusters, N fastest (neighbouring clusters reuse the same activation tiles in L2).
+  // Tile schedule: a "pair" = CL consecutive M tiles x one N tile; pairs are dealt round-robin to clusters, N fastest
+  // (neighbouring clusters reuse the same activation tiles in L2).  With CL == 2 the second M tile of the last pair
+  // may lie past the grid: its loads zero-fill and its stores are clipped.
   const uint32_t cta_rank = CL > 1 ? cluster_ctarank() : 0u;
   const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int m_pairs = (m_tiles + CL - 1) / CL;
-  const int total_pairs = m_pairs * p.n_tiles;
+  const int total = (m_tiles + CL - 1) / CL * p.n_tiles;
   const int cluster_id = blockIdx.x / CL, n_clusters = gridDim.x / CL;
   constexpr int kBN64 = (BN + 63) / 64;
   constexpr uint16_t kMcMask = (uint16_t)((1u << CL) - 1u);
 
   if (warp == 0) {
     // ===================== TMA producer (converged warp, one elected lane issues) =====================
-    {
-      int stage = 0; uint32_t phase = 0;
-      for (int pair = cluster_id; pair < total_pairs; pair += n_clusters) {
-        const int n_tile = pair % p.n_tiles;
-        const int m_tile = (pair / p.n_tiles) * CL + (int)cta_rank;   // may exceed m_tiles: loads zero-fill, stores clip
-        const int tw = m_tile % p.tiles_w;
-        const int th = (m_tile / p.tiles_w) % p.tiles_h;
-        const int tn = m_tile / (p.tiles_w * p.tiles_h);
-        const bool masked = build_live_mask<kBN64>(p, n_tile, lane, live_prod);
-        int j = 0;
-        for (int t = 0; t < p.ntaps; ++t) {
-          const TapInfo tap = p.taps[t];
-          for (int kb = 0; kb < p.kblks; ++kb, ++j) {
-            if (masked && !((live_prod[j >> 5] >> (j & 31)) & 1u)) continue;
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            if (elect_one()) {
-              const uint32_t a_dst = smem_base + stage * kStageBytes;
-              const uint32_t b_dst = a_dst + kABytes;
-              mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
-              tma_load_4d(a_dst, &amaps.a[tap.map_id], full_bar(stage), kb * kBK, tw * p.bw + tap.dw,
-                          th * p.bh + tap.dh, tn * p.bn);
-              if (CL > 1) {     // my half of the weight tile, multicast to every CTA of the cluster
-                tma_load_3d_mc(b_dst + cta_rank * (uint32_t)(BN / CL) * 128u, &bmap, full_bar(stage), kb * kBK,
-                               n_tile * BN + (int)cta_rank * (BN / CL), tap.b_tap, kMcMask);
-              } else {
-                tma_load_3d(b_dst, &bmap, full_bar(stage), kb * kBK, n_tile * BN, tap.b_tap);
-              }
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // The whole warp runs the loop converged and ONE ELECTED lane issues: with an elect.sync
-    // predicate the descriptors stay in uniform registers (a `lane == 0` test costs ~13 extra
-    // instructions per MMA, more than a 128 x 64 x 16 MMA takes to execute).
-    {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int pair = cluster_id; pair < total_pairs; pair += n_clusters) {
-        const int n_tile = pair % p.n_tiles;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);       // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        const bool masked = build_live_mask<kBN64>(p, n_tile, lane, live_mma);
-        bool first = true;
-        const int nkb = p.ntaps * p.kblks;
-        for (int j = 0; j < nkb; ++j) {
-          if (masked && !((live_mma[j >> 5] >> (j & 31)) & 1u)) continue;
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint64_t da = make_smem_desc(smem_base + stage * kStageBytes, 16, 1024);
-            const uint64_t db = make_smem_desc(smem_base + stage * kStageBytes + kABytes, 16, 1024);
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k)          // +32 bytes along K = +2 in the 16-byte address field
-              umma_bf16(d_tmem, da + 2 * k, db + 2 * k, kIdesc, (first && k == 0) ? 0u : 1u);
-            if (CL > 1) umma_commit_mc(empty_bar(stage), kMcMask);   // release the slot in BOTH CTAs
-            else umma_commit(empty_bar(stage));          // frees the smem slot when the MMAs retire
-          }
-          __syncwarp();
-          first = false;
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        if (elect_one()) umma_commit(tfull_bar(acc));      // accumulator complete
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int quad = warp & 3;                            // TMEM lane quadrant this warp may read
-    const int row = quad * 32 + lane;                     // pixel index inside the box
-    int acc = 0; uint32_t acc_phase = 0;
-    uint32_t slab_ctr = 0;
-    float* bn_row = p.bn_partial ? p.bn_partial + (size_t)blockIdx.x * 2 * p.N : nullptr;
-    if (bn_row) {            // this CTA's row of the batch-norm partial sums starts at zero
-      for (int i = (warp - 2) * 32 + lane; i < 2 * p.N; i += 128) bn_row[i] = 0.f;
-      __threadfence_block();
-      named_bar_sync(1, 128);
-    }
-    for (int pair = cluster_id; pair < total_pairs; pair += n_clusters) {
-      const int n_tile = pair % p.n_tiles;
-      const int m_tile = (pair / p.n_tiles) * CL + (int)cta_rank;
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = cluster_id; tile < total; tile += n_clusters) {
+      const int n_tile = tile % p.n_tiles;
+      const int m_tile = (tile / p.n_tiles) * CL + (int)cta_rank;
       const int tw = m_tile % p.tiles_w;
       const int th = (m_tile / p.tiles_w) % p.tiles_h;
       const int tn = m_tile / (p.tiles_w * p.tiles_h);
-      const int pw = tw * p.bw + row % p.bw;
-      const int ph = th * p.bh + (row / p.bw) % p.bh;
-      const int pn = tn * p.bn + row / (p.bw * p.bh);
-      const bool pix_ok = pw < p.GW && ph < p.GH && pn < p.NB;
-      const long long o_pix = p.o_off + pn * p.o_sn + ph * p.o_sh + pw * p.o_sw;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
+      const bool masked = build_live_mask<kBN64>(p, n_tile, lane, live_prod);
+      int j = 0;
+      for (int t = 0; t < p.ntaps; ++t) {
+        const TapInfo tap = p.taps[t];
+        for (int kb = 0; kb < p.kblks; ++kb, ++j) {
+          if (masked && !((live_prod[j >> 5] >> (j & 31)) & 1u)) continue;
+          if (CL > 1) mbar_wait_cluster(empty_bar(stage), phase ^ 1u);
+          else mbar_wait(empty_bar(stage), phase ^ 1u);
+          if (elect_one()) {
+            const uint32_t a_dst = smem_base + stage * kStageBytes;
+            mbar_arrive_expect_tx(full_bar(stage), kStageBytes);      // my A + both halves of B
+            tma_load_4d(a_dst, &amaps.a[tap.map_id], full_bar(stage), kb * kBK, tw * p.bw + tap.dw,
+                        th * p.bh + tap.dh, tn * p.bn);
+            if (CL > 1)        // my half of the weight tile, multicast to every CTA of the cluster
+              tma_load_3d_mc(a_dst + kABytes + cta_rank * (uint32_t)(BN / CL) * 128u, &bmap, full_bar(stage),
+                             kb * kBK, n_tile * BN + (int)cta_rank * (BN / CL), tap.b_tap, kMcMask);
+            else
+              tma_load_3d(a_dst + kABytes, &bmap, full_bar(stage), kb * kBK, n_tile * BN, tap.b_tap);
+          }
+          __syncwarp();
+          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+  } else if (warp >= kConsumerWarp0) {
+    // ===================== consumers: wgmma main loop + epilogue =====================
+    const int cw = warp - kConsumerWarp0;                 // 0..7
+    const int wg = cw >> 2;                               // 64-row half of the tile
+    const int row = 64 * wg + 16 * (cw & 3) + (lane >> 2);   // this thread's first tile row (second: row + 8)
+    const bool issuer = (cw == 0 && lane == 0);
+    float acc[BN / 2];
+    int stage = 0; uint32_t phase = 0;
+    uint32_t slab_ctr = 0;
+    float* bn_row = p.bn_partial ? p.bn_partial + (size_t)blockIdx.x * 2 * p.N : nullptr;
+    if (bn_row) {            // this CTA's row of the batch-norm partial sums starts at zero
+      for (int i = cw * 32 + lane; i < 2 * p.N; i += kConsumerThreads) bn_row[i] = 0.f;
+      __threadfence_block();
+      named_bar_sync(1, kConsumerThreads);
+    }
+    int tile_ctr = 0;
+    for (int tile = cluster_id; tile < total; tile += n_clusters, ++tile_ctr) {
+      const int n_tile = tile % p.n_tiles;
+      const int m_tile = (tile / p.n_tiles) * CL + (int)cta_rank;
+      // the first warp of the warpgroup builds the tile's liveness mask, the other three wait for it
+      uint32_t* live = live_cons[wg][tile_ctr & 1];
+      if ((cw & 3) == 0) build_live_mask<kBN64>(p, n_tile, lane, live);
+      named_bar_sync(3 + wg, 128);
+      const bool masked = live_mask_used(p);
+      zero_acc(acc);
+      int prev = -1;
+      const int nkb = p.ntaps * p.kblks;
+      for (int j = 0; j < nkb; ++j) {
+        if (masked && !((live[j >> 5] >> (j & 31)) & 1u)) continue;
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t a_src = smem_base + stage * kStageBytes;
+        const uint64_t da = make_smem_desc(a_src + (uint32_t)wg * 64u * 128u, 16, 1024);
+        const uint64_t db = make_smem_desc(a_src + kABytes, 16, 1024);
+        fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k)              // +32 bytes along K = +2 in the 16-byte address field
+          Wgmma<BN>::template ss<0, 0>(acc, da + 2 * k, db + 2 * k);
+        wgmma_commit();
+        wgmma_wait<1>();                                  // the previous stage's MMAs have read their operands
+        if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+
+      const int tw = m_tile % p.tiles_w;
+      const int th = (m_tile / p.tiles_w) % p.tiles_h;
+      const int tn = m_tile / (p.tiles_w * p.tiles_h);
+      bool ok[2]; long long o_pix[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = row + 8 * h;
+        const int pw = tw * p.bw + r % p.bw;
+        const int ph = th * p.bh + (r / p.bw) % p.bh;
+        const int pn = tn * p.bn + r / (p.bw * p.bh);
+        ok[h] = pw < p.GW && ph < p.GH && pn < p.NB;
+        o_pix[h] = p.o_off + pn * p.o_sn + ph * p.o_sh + pw * p.o_sw;
+      }
       if (p.tma_store) {
         // ---- stage 64-channel slabs in smem (128B-swizzled rows) and TMA-store them ----
-        const bool issuer = (warp == 2 && lane == 0);
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 64) {
-          const int co0 = n_tile * BN + c0;
+#pragma unroll
+        for (int s = 0; s < kBN64; ++s) {
+          const int co0 = n_tile * BN + 64 * s;
           if (co0 >= p.N) break;                                   // uniform: whole slab out of range
           const uint32_t slab = out_base + (uint32_t)(slab_ctr & 1) * kSlabBytes;
           if (issuer) tma_store_wait_read<1>();                    // the store that last used this slab is done reading
-          named_bar_sync(1, 128);
-          uint32_t r0[32], r1[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c0), r0);
-          tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c0 + 32), r1);
-          tmem_ld_wait();
-          const uint32_t row_addr = slab + (uint32_t)row * 128u;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int e = 8 * j + 2 * q;
-              const float a = __uint_as_float(e < 32 ? r0[e] : r1[e - 32]);
-              const float b = __uint_as_float(e + 1 < 32 ? r0[e + 1] : r1[e + 1 - 32]);
-              __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-              pk[q] = pix_ok ? *reinterpret_cast<uint32_t*>(&h) : 0u;   // rows outside the grid: clipped by the
-            }                                                           // store, must be zero for the statistics
-            const uint32_t dst = row_addr + (uint32_t)((j ^ (row & 7)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]),
-                         "r"(pk[3])
-                         : "memory");
-          }
+          named_bar_sync(1, kConsumerThreads);
+          if (s == 0) stage_slab<0>(acc, slab, row, ok[0], ok[1], lane);
+          else stage_slab<(kBN64 > 1 ? 1 : 0)>(acc, slab, row, ok[0], ok[1], lane);
           fence_proxy_async_smem();
-          named_bar_sync(1, 128);
+          named_bar_sync(1, kConsumerThreads);
           if (issuer) {
             tma_store_4d(&omap, slab, co0, tw * p.bw, th * p.bh, tn * p.bn);
             tma_store_commit();
           }
-          if (bn_row) slab_bn_stats(slab, quad, lane, bn_row, co0, p.N, p.stats_dbg);   // next to the bulk store's own read
+          if (bn_row && wg == 0) slab_bn_stats(slab, cw, lane, bn_row, co0, p.N, p.stats_dbg);   // next to the bulk store's own read
           ++slab_ctr;
         }
       } else {
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c0), r);
-        tmem_ld_wait();
-        const int co0 = n_tile * BN + c0;
-        if (pix_ok && co0 < p.N) {
-          if (p.out_bf16) {
-            __nv_bfloat16* dst = p.out_bf16 + o_pix + co0;
+        // direct global stores (fp32 output / bias: the dense layer)
 #pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              if (co0 + j + 8 <= p.N) {
-                uint32_t pk[4];
+        for (int jc = 0; jc < BN / 8; ++jc) {
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  float a = __uint_as_float(r[j + 2 * q]), b = __uint_as_float(r[j + 2 * q + 1]);
-                  if (p.bias) { a += __ldg(p.bias + co0 + j + 2 * q); b += __ldg(p.bias + co0 + j + 2 * q + 1); }
-                  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-                  pk[q] = *reinterpret_cast<uint32_t*>(&h);
-                }
-                *reinterpret_cast<uint4*>(dst + j) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-              } else {
-                for (int q = 0; q < 8 && co0 + j + q < p.N; ++q) {
-                  float a = __uint_as_float(r[j + q]);
-                  if (p.bias) a += __ldg(p.bias + co0 + j + q);
-                  dst[j + q] = __float2bfloat16(a);
-                }
-              }
-            }
-          }
-          if (p.out_f32) {
-            float* dst = p.out_f32 + o_pix + co0;
+          for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              if (co0 + j + 4 <= p.N) {
-                float4 v = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                       __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-                if (p.bias) {
-                  v.x += __ldg(p.bias + co0 + j); v.y += __ldg(p.bias + co0 + j + 1);
-                  v.z += __ldg(p.bias + co0 + j + 2); v.w += __ldg(p.bias + co0 + j + 3);
-                }
-                *reinterpret_cast<float4*>(dst + j) = v;
-              } else {
-                for (int q = 0; q < 4 && co0 + j + q < p.N; ++q) {
-                  float a = __uint_as_float(r[j + q]);
-                  if (p.bias) a += __ldg(p.bias + co0 + j + q);
-                  dst[j + q] = a;
-                }
+            for (int e = 0; e < 2; ++e) {
+              const int co = n_tile * BN + 8 * jc + 2 * (lane & 3) + e;
+              if (ok[h] && co < p.N) {
+                float a = acc[4 * jc + 2 * h + e];
+                if (p.bias) a += __ldg(p.bias + co);
+                if (p.out_bf16) p.out_bf16[o_pix[h] + co] = __float2bfloat16(a);
+                if (p.out_f32) p.out_f32[o_pix[h] + co] = a;
               }
             }
           }
         }
       }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
     }
-    if (p.tma_store && warp == 2 && lane == 0) tma_store_wait_all();   // smem must outlive the bulk stores
+    if (p.tma_store && issuer) tma_store_wait_all();   // smem must outlive the bulk stores
   }
-  tc_fence_before();
-  if (CL > 1) cluster_sync_all(); else __syncthreads();    // no CTA exits while a peer may still signal it
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
+  if (CL > 1) cluster_sync_all();                         // no CTA exits while its peer may still signal it
 }
 
 // ----------------------------------------------------------------------------
@@ -434,271 +396,10 @@ struct WgradParams {
   float beta;                       // dw <- beta * dw + sum of the partials
 };
 
-// ----------------------------------------------------------------------------
-// CTA-pair version of the fprop / dgrad kernel: tcgen05.mma.cta_group::2, M = 256.
-// A single SM cannot feed its tensor core from shared memory at full rate with a 128 x N x 64
-// tile (per K block it writes A+B once and reads them once: ~190 B/clk against a 128 B/clk smem
-// port).  With cta_group::2 the two SMs of a TPC compute ONE 256 x N tile: each holds its own
-// 128 pixel rows of A and only HALF of the weight tile, so the per-SM smem traffic per FLOP drops
-// by a third and the instruction count halves.  Protocol (as CUTLASS / the Blackwell guide):
-//   * both CTAs' TMA loads (.cta_group::2) complete on the LEADER's full barrier
-//     (count 2: leader's arrive.expect_tx for both halves + the peer's remote arrive);
-//   * only the leader issues MMAs; tcgen05.commit.cta_group::2 multicasts the "slot free" and
-//     "accumulator ready" arrivals to both CTAs;
-//   * each CTA's epilogue drains its own 128 TMEM lanes and arrives on the leader's
-//     "accumulator free" barrier (count 8).
-// ----------------------------------------------------------------------------
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(kThreads, 1)
-k_igemm_kmajor2(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
-                const __grid_constant__ CUtensorMap omap, const IgemmParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr uint32_t kABytes = kBM * kBK * 2;              // my 128 pixel rows: 16 KB
-  constexpr uint32_t kBBytes = (BN / 2) * kBK * 2;          // my half of the weight tile
-  constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  constexpr uint32_t kIdesc = make_idesc_bf16(2 * kBM, BN, 0, 0);
-  constexpr uint32_t kSlabBytes = kBM * 64 * 2;
-  constexpr uint16_t kPairMask = 0x3;
-
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t out_base = smem_base + STAGES * kStageBytes;
-  const uint32_t bar_base = out_base + 2 * kSlabBytes;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  auto peer_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 6 + s); };   // leader: the peer's tile has landed
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  __shared__ uint32_t live_prod[kLiveWords], live_mma[kLiveWords];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t cta_rank = cluster_ctarank();
-  const bool leader = cta_rank == 0;
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < 4; ++i) prefetch_tmap(&amaps.a[i]);
-    prefetch_tmap(&bmap);
-    if (p.tma_store) prefetch_tmap(&omap);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), p.pair_local ? 1 : 2); mbar_init(empty_bar(s), 1); mbar_init(peer_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 8); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2cta(tmem_slot, kTmemCols);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int m_pairs = (m_tiles + 1) / 2;
-  const int total_pairs = m_pairs * p.n_tiles;
-  const int cluster_id = blockIdx.x / 2, n_clusters = gridDim.x / 2;
-  constexpr int kBN64 = (BN + 63) / 64;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs; converged warp, one elected lane issues) =====================
-    {
-      int stage = 0; uint32_t phase = 0;
-      for (int pair = cluster_id; pair < total_pairs; pair += n_clusters) {
-        const int n_tile = pair % p.n_tiles;
-        const int m_tile = (pair / p.n_tiles) * 2 + (int)cta_rank;
-        const int tw = m_tile % p.tiles_w;
-        const int th = (m_tile / p.tiles_w) % p.tiles_h;
-        const int tn = m_tile / (p.tiles_w * p.tiles_h);
-        const bool masked = build_live_mask<kBN64>(p, n_tile, lane, live_prod);
-        int j = 0;
-        for (int t = 0; t < p.ntaps; ++t) {
-          const TapInfo tap = p.taps[t];
-          for (int kb = 0; kb < p.kblks; ++kb, ++j) {
-            if (masked && !((live_prod[j >> 5] >> (j & 31)) & 1u)) continue;
-            mbar_wait(empty_bar(stage), phase ^ 1u);
-            if (elect_one()) {
-              const uint32_t a_dst = smem_base + stage * kStageBytes;
-              const uint32_t b_dst = a_dst + kABytes;
-              if (p.pair_local) {
-                // Each CTA's bytes complete on its OWN barrier; the peer's idle MMA warp forwards ONE
-                // cluster-scope arrive per stage to the leader.  (With the loads of both CTAs signalling the
-                // leader's barrier the peer's TMA stream only reached ~33 of the 54 B/clk a lone SM ingests.)
-                mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
-                tma_load_4d(a_dst, &amaps.a[tap.map_id], full_bar(stage), kb * kBK, tw * p.bw + tap.dw,
-                            th * p.bh + tap.dh, tn * p.bn);
-                tma_load_3d(b_dst, &bmap, full_bar(stage), kb * kBK, n_tile * BN + (int)cta_rank * (BN / 2), tap.b_tap);
-              } else {
-                if (leader) mbar_arrive_expect_tx(full_bar(stage), 2 * kStageBytes);   // both CTAs' bytes land here
-                else mbar_arrive_leader(full_bar(stage));
-                tma_load_4d_2cta(a_dst, &amaps.a[tap.map_id], full_bar(stage), kb * kBK, tw * p.bw + tap.dw,
-                                 th * p.bh + tap.dh, tn * p.bn);
-                tma_load_3d_2cta(b_dst, &bmap, full_bar(stage), kb * kBK, n_tile * BN + (int)cta_rank * (BN / 2),
-                                 tap.b_tap);
-              }
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only; converged warp, one elected lane) =====================
-    if (leader) {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int pair = cluster_id; pair < total_pairs; pair += n_clusters) {
-        const int n_tile = pair % p.n_tiles;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);       // both epilogues have drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        const bool masked = build_live_mask<kBN64>(p, n_tile, lane, live_mma);
-        bool first = true;
-        const int nkb = p.ntaps * p.kblks;
-        for (int j = 0; j < nkb; ++j) {
-          if (masked && !((live_mma[j >> 5] >> (j & 31)) & 1u)) continue;
-          mbar_wait(full_bar(stage), phase);
-          if (p.pair_local) mbar_wait_cluster(peer_bar(stage), phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint64_t da = make_smem_desc(smem_base + stage * kStageBytes, 16, 1024);
-            const uint64_t db = make_smem_desc(smem_base + stage * kStageBytes + kABytes, 16, 1024);
-#pragma unroll
-            for (int k = 0; k < kBK / 16; ++k)
-              umma_bf16_2cta(d_tmem, da + 2 * k, db + 2 * k, kIdesc, (first && k == 0) ? 0u : 1u);
-            umma_commit_2cta_mc(empty_bar(stage), kPairMask);     // slot free in BOTH CTAs
-          }
-          __syncwarp();
-          first = false;
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        if (elect_one()) umma_commit_2cta_mc(tfull_bar(acc), kPairMask);   // accumulator ready in BOTH CTAs
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-    else if (p.pair_local) {
-      // ===== peer CTA: forward "my tile of this stage has landed" to the leader, one arrive per stage =====
-      int stage = 0; uint32_t phase = 0;
-      for (int pair = cluster_id; pair < total_pairs; pair += n_clusters) {
-        const int n_tile = pair % p.n_tiles;
-        const bool masked = build_live_mask<kBN64>(p, n_tile, lane, live_mma);
-        const int nkb = p.ntaps * p.kblks;
-        for (int j = 0; j < nkb; ++j) {
-          if (masked && !((live_mma[j >> 5] >> (j & 31)) & 1u)) continue;
-          mbar_wait(full_bar(stage), phase);
-          if (elect_one()) mbar_arrive_leader_release(peer_bar(stage));
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..5 of both CTAs) =====================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
-    uint32_t slab_ctr = 0;
-    float* bn_row = p.bn_partial ? p.bn_partial + (size_t)blockIdx.x * 2 * p.N : nullptr;
-    if (bn_row) {            // this CTA's row of the batch-norm partial sums starts at zero
-      for (int i = (warp - 2) * 32 + lane; i < 2 * p.N; i += 128) bn_row[i] = 0.f;
-      __threadfence_block();
-      named_bar_sync(1, 128);
-    }
-    for (int pair = cluster_id; pair < total_pairs; pair += n_clusters) {
-      const int n_tile = pair % p.n_tiles;
-      const int m_tile = (pair / p.n_tiles) * 2 + (int)cta_rank;
-      const int tw = m_tile % p.tiles_w;
-      const int th = (m_tile / p.tiles_w) % p.tiles_h;
-      const int tn = m_tile / (p.tiles_w * p.tiles_h);
-      const int pw = tw * p.bw + row % p.bw;
-      const int ph = th * p.bh + (row / p.bw) % p.bh;
-      const int pn = tn * p.bn + row / (p.bw * p.bh);
-      const bool pix_ok = pw < p.GW && ph < p.GH && pn < p.NB;
-      const long long o_pix = p.o_off + pn * p.o_sn + ph * p.o_sh + pw * p.o_sw;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const bool issuer = (warp == 2 && lane == 0);
-      if (p.tma_store) {
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 64) {
-          const int co0 = n_tile * BN + c0;
-          if (co0 >= p.N) break;
-          const uint32_t slab = out_base + (uint32_t)(slab_ctr & 1) * kSlabBytes;
-          if (issuer) tma_store_wait_read<1>();
-          named_bar_sync(1, 128);
-          uint32_t r0[32], r1[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c0), r0);
-          tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c0 + 32), r1);
-          tmem_ld_wait();
-          const uint32_t row_addr = slab + (uint32_t)row * 128u;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int e = 8 * j + 2 * q;
-              const float a = __uint_as_float(e < 32 ? r0[e] : r1[e - 32]);
-              const float b = __uint_as_float(e + 1 < 32 ? r0[e + 1] : r1[e + 1 - 32]);
-              __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-              pk[q] = pix_ok ? *reinterpret_cast<uint32_t*>(&h) : 0u;   // rows outside the grid: clipped by the
-            }                                                           // store, must be zero for the statistics
-            const uint32_t dst = row_addr + (uint32_t)((j ^ (row & 7)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]),
-                         "r"(pk[3])
-                         : "memory");
-          }
-          fence_proxy_async_smem();
-          named_bar_sync(1, 128);
-          if (issuer) {
-            tma_store_4d(&omap, slab, co0, tw * p.bw, th * p.bh, tn * p.bn);
-            tma_store_commit();
-          }
-          if (bn_row) slab_bn_stats(slab, quad, lane, bn_row, co0, p.N, p.stats_dbg);   // next to the bulk store's own read
-          ++slab_ctr;
-        }
-      } else {
-        // direct global stores (fp32 output / bias: the dense layer); static register indexing only
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c0), r);
-          tmem_ld_wait();
-          const int co0 = n_tile * BN + c0;
-          if (pix_ok && co0 < p.N) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              if (co0 + j < p.N) {
-                float a = __uint_as_float(r[j]);
-                if (p.bias) a += __ldg(p.bias + co0 + j);
-                if (p.out_bf16) p.out_bf16[o_pix + co0 + j] = __float2bfloat16(a);
-                if (p.out_f32) p.out_f32[o_pix + co0 + j] = a;
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) mbar_arrive(tempty_bar(acc));
-        else mbar_arrive_leader(tempty_bar(acc));
-      }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
-    if (p.tma_store && warp == 2 && lane == 0) tma_store_wait_all();
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, kTmemCols);
-  }
-}
-
-// CL = CTAs per cluster (1 or 2).  The dY tile depends only on (pixel block, N tile), so with
-// CL == 2 two work units that differ in (tap, M tile) share it: each CTA fetches half of the dY
-// boxes and multicasts them to both (same protocol as k_igemm_kmajor).
+// Same warp roles as k_igemm_kmajor; consumer warpgroup w owns input channels 64w..64w+63 of the unit (the
+// w-th 64-channel x box of a stage is its whole A operand).  CL = CTAs per cluster (1 or 2): the dY tile depends only
+// on (pixel block, N tile), so with CL == 2 two work units that differ in (tap, M tile) share it; each CTA fetches
+// half of the dY boxes and multicasts them to both (same protocol as k_igemm_kmajor).
 template <int BN, int STAGES, int CL>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUtensorMap dymap,
@@ -708,8 +409,6 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
   constexpr uint32_t kBBytes = BN * kBK * 2;
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
   constexpr uint32_t kBox = 64 * 64 * 2;             // 8 KB: 64 pixels x 64 channels
-  constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  constexpr uint32_t kIdesc = make_idesc_bf16(kBM, BN, 1, 1);
   constexpr int kBBoxes = BN / 64;
   static_assert(CL == 1 || kBBoxes % CL == 0, "multicast splits the dY boxes between the CTAs");
   constexpr uint16_t kMcMask = (uint16_t)((1u << CL) - 1u);
@@ -718,30 +417,20 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
   const uint32_t bar_base = smem_base + STAGES * kStageBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   __shared__ int s_last;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int i = 0; i < 4; ++i) prefetch_tmap(&xmaps.a[i]);
     prefetch_tmap(&dymap);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CL); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps * CL); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   if (CL > 1) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  // Work units: (split, N tile, M index) with M index = tap * m_tiles + m_tile; a cluster takes
-  // CL consecutive M indices of one (split, N tile).  Indices past the end are idle partners:
-  // their x boxes are requested out of bounds (zero fill) and nothing is stored.
+  // Work units: (split, N tile, M index) with M index = tap * m_tiles + m_tile; a cluster takes CL consecutive M
+  // indices of one (split, N tile).  Indices past the end are idle partners: their x boxes are requested out of
+  // bounds (zero fill) and nothing is stored.
   const uint32_t cta_rank = CL > 1 ? cluster_ctarank() : 0u;
   const int mcount = p.ntaps * p.m_tiles;
   const int m_groups = (mcount + CL - 1) / CL;
@@ -750,84 +439,54 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
   const int cluster_id = blockIdx.x / CL, n_clusters = gridDim.x / CL;
 
   if (warp == 0) {
-    {                                                      // converged warp, one elected lane issues
-      int stage = 0; uint32_t phase = 0;
-      for (int q = cluster_id; q < total_groups; q += n_clusters) {
-        const int split = q / groups_per_split;
-        const int r = q % groups_per_split;
-        const int n_tile = r % p.n_tiles;
-        const int mi = (r / p.n_tiles) * CL + (int)cta_rank;
-        const bool live = mi < mcount;
-        const TapInfo tap = p.taps[live ? mi / p.m_tiles : 0];
-        const int c_base = live ? (mi % p.m_tiles) * kBM : (1 << 28);     // idle partner: out of bounds
-        const int pb0 = split * p.pblocks_per_split;
-        const int pb1 = min(pb0 + p.pblocks_per_split, p.pblocks);
-        int tw = pb0 % p.tiles_w, th = (pb0 / p.tiles_w) % p.tiles_h, tn = pb0 / (p.tiles_w * p.tiles_h);
-        for (int pb = pb0; pb < pb1; ++pb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          if (elect_one()) {
-            const uint32_t a_dst = smem_base + stage * kStageBytes;
-            const uint32_t b_dst = a_dst + kABytes;
-            mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
+    int stage = 0; uint32_t phase = 0;                     // converged warp, one elected lane issues
+    for (int q = cluster_id; q < total_groups; q += n_clusters) {
+      const int split = q / groups_per_split;
+      const int r = q % groups_per_split;
+      const int n_tile = r % p.n_tiles;
+      const int mi = (r / p.n_tiles) * CL + (int)cta_rank;
+      const bool live = mi < mcount;
+      const TapInfo tap = p.taps[live ? mi / p.m_tiles : 0];
+      const int c_base = live ? (mi % p.m_tiles) * kBM : (1 << 28);     // idle partner: out of bounds
+      const int pb0 = split * p.pblocks_per_split;
+      const int pb1 = min(pb0 + p.pblocks_per_split, p.pblocks);
+      int tw = pb0 % p.tiles_w, th = (pb0 / p.tiles_w) % p.tiles_h, tn = pb0 / (p.tiles_w * p.tiles_h);
+      for (int pb = pb0; pb < pb1; ++pb) {
+        if (CL > 1) mbar_wait_cluster(empty_bar(stage), phase ^ 1u);
+        else mbar_wait(empty_bar(stage), phase ^ 1u);
+        if (elect_one()) {
+          const uint32_t a_dst = smem_base + stage * kStageBytes;
+          const uint32_t b_dst = a_dst + kABytes;
+          mbar_arrive_expect_tx(full_bar(stage), kStageBytes);
 #pragma unroll
-            for (int h = 0; h < kBM / 64; ++h)
-              tma_load_4d(a_dst + h * kBox, &xmaps.a[tap.map_id], full_bar(stage), c_base + h * 64,
-                          tw * p.bw + tap.dw, th * p.bh + tap.dh, tn * p.bn);
-            if (CL > 1) {
+          for (int h = 0; h < kBM / 64; ++h)
+            tma_load_4d(a_dst + h * kBox, &xmaps.a[tap.map_id], full_bar(stage), c_base + h * 64,
+                        tw * p.bw + tap.dw, th * p.bh + tap.dh, tn * p.bn);
+          if (CL > 1) {
 #pragma unroll
-              for (int hh = 0; hh < kBBoxes / CL; ++hh) {
-                const int h = (int)cta_rank * (kBBoxes / CL) + hh;
-                tma_load_4d_mc(b_dst + h * kBox, &dymap, full_bar(stage), n_tile * BN + h * 64, tw * p.bw,
-                               th * p.bh, tn * p.bn, kMcMask);
-              }
-            } else {
-#pragma unroll
-              for (int h = 0; h < kBBoxes; ++h)
-                tma_load_4d(b_dst + h * kBox, &dymap, full_bar(stage), n_tile * BN + h * 64, tw * p.bw,
-                            th * p.bh, tn * p.bn);
+            for (int hh = 0; hh < kBBoxes / CL; ++hh) {
+              const int h = (int)cta_rank * (kBBoxes / CL) + hh;
+              tma_load_4d_mc(b_dst + h * kBox, &dymap, full_bar(stage), n_tile * BN + h * 64, tw * p.bw,
+                             th * p.bh, tn * p.bn, kMcMask);
             }
-          }
-          __syncwarp();
-          if (++tw == p.tiles_w) { tw = 0; if (++th == p.tiles_h) { th = 0; ++tn; } }   // next pixel block (no divisions)
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    {                                                      // converged warp, one elected lane issues
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int q = cluster_id; q < total_groups; q += n_clusters) {
-        const int split = q / groups_per_split;
-        const int pb0 = split * p.pblocks_per_split;
-        const int pb1 = min(pb0 + p.pblocks_per_split, p.pblocks);
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int pb = pb0; pb < pb1; ++pb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint64_t da = make_smem_desc(smem_base + stage * kStageBytes, kBox, 1024);
-            const uint64_t db = make_smem_desc(smem_base + stage * kStageBytes + kABytes, kBox, 1024);
+          } else {
 #pragma unroll
-            for (int k = 0; k < kBK / 16; ++k)            // 16 pixels = 16 rows of 128 B = +128 address units
-              umma_bf16(d_tmem, da + 128 * k, db + 128 * k, kIdesc, (pb == pb0 && k == 0) ? 0u : 1u);
-            if (CL > 1) umma_commit_mc(empty_bar(stage), kMcMask);
-            else umma_commit(empty_bar(stage));
+            for (int h = 0; h < kBBoxes; ++h)
+              tma_load_4d(b_dst + h * kBox, &dymap, full_bar(stage), n_tile * BN + h * 64, tw * p.bw,
+                          th * p.bh, tn * p.bn);
           }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
-        if (elect_one()) umma_commit(tfull_bar(acc));
         __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+        if (++tw == p.tiles_w) { tw = 0; if (++th == p.tiles_h) { th = 0; ++tn; } }   // next pixel block (no divisions)
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
     }
-  } else {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    int acc = 0; uint32_t acc_phase = 0;
+  } else if (warp >= kConsumerWarp0) {
+    const int cw = warp - kConsumerWarp0;
+    const int wg = cw >> 2;
+    const int row = 64 * wg + 16 * (cw & 3) + (lane >> 2);
+    float acc[BN / 2];
+    int stage = 0; uint32_t phase = 0;
     for (int q = cluster_id; q < total_groups; q += n_clusters) {
       const int split = q / groups_per_split;
       const int r = q % groups_per_split;
@@ -835,41 +494,51 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
       const int mi = (r / p.n_tiles) * CL + (int)cta_rank;
       const bool live = mi < mcount;
       const int tap_idx = live ? mi / p.m_tiles : 0;
-      const int ci = live ? (mi % p.m_tiles) * kBM + row : p.ci;          // idle partner stores nothing
-      float* dst_row = p.out + (long long)split * p.split_stride +
-                       ((long long)p.taps[tap_idx].b_tap * p.ci + ci) * p.co;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t r32[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * BN + c0), r32);
-        tmem_ld_wait();
-        const int co0 = n_tile * BN + c0;
-        if (ci < p.ci && co0 < p.co) {
+      const int pb0 = split * p.pblocks_per_split;
+      const int pb1 = min(pb0 + p.pblocks_per_split, p.pblocks);
+      zero_acc(acc);
+      int prev = -1;
+      for (int pb = pb0; pb < pb1; ++pb) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t a_src = smem_base + stage * kStageBytes;
+        const uint64_t da = make_smem_desc(a_src + (uint32_t)wg * kBox, kBox, 1024);
+        const uint64_t db = make_smem_desc(a_src + kABytes, kBox, 1024);
+        fence_regs(acc);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            if (co0 + j + 4 <= p.co) {
-              *reinterpret_cast<float4*>(dst_row + co0 + j) =
-                  make_float4(__uint_as_float(r32[j]), __uint_as_float(r32[j + 1]), __uint_as_float(r32[j + 2]),
-                              __uint_as_float(r32[j + 3]));
-            } else {
-              for (int t = 0; t < 4 && co0 + j + t < p.co; ++t) dst_row[co0 + j + t] = __uint_as_float(r32[j + t]);
-            }
-          }
+        for (int k = 0; k < kBK / 16; ++k)              // 16 pixels = 16 rows of 128 B = +128 address units
+          Wgmma<BN>::template ss<1, 1>(acc, da + 128 * k, db + 128 * k);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+
+      const int m0 = live ? (mi % p.m_tiles) * kBM : p.ci;            // idle partner stores nothing
+      float* base = p.out + (long long)split * p.split_stride + (long long)p.taps[tap_idx].b_tap * p.ci * p.co;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int ci = m0 + row + 8 * h;
+        if (ci >= p.ci) continue;
+#pragma unroll
+        for (int jc = 0; jc < BN / 8; ++jc) {
+          const int co = n_tile * BN + 8 * jc + 2 * (lane & 3);          // co is even and p.co % 8 == 0
+          if (co < p.co)
+            *reinterpret_cast<float2*>(base + (long long)ci * p.co + co) =
+                make_float2(acc[4 * jc + 2 * h], acc[4 * jc + 2 * h + 1]);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
       if (p.counters != nullptr) {
         // ---- split-K fix-up inside the kernel: the unit that arrives LAST at an output tile sums the partial
         // tiles of all splits in split order (deterministic) while they are still in L2, and writes dw.  Replaces
         // one k_splitk_reduce launch per layer.
         __threadfence();                                   // my part of this unit's partial tile is visible
-        named_bar_sync(2, 128);
-        if (warp == 2 && lane == 0) {
+        named_bar_sync(2, kConsumerThreads);
+        if (cw == 0 && lane == 0) {
           int last = 0;
           if (live) {
             int* ctr = p.counters + (mi * p.n_tiles + n_tile);
@@ -878,12 +547,11 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
           }
           s_last = last;
         }
-        named_bar_sync(2, 128);
+        named_bar_sync(2, kConsumerThreads);
         if (s_last) {
           __threadfence();
-          const int m0 = (mi % p.m_tiles) * kBM;
           const long long tap_off = (long long)p.taps[tap_idx].b_tap * p.ci;
-          for (int rr = warp - 2; rr < kBM && m0 + rr < p.ci; rr += 4) {       // warp per row, lanes over columns
+          for (int rr = cw; rr < kBM && m0 + rr < p.ci; rr += kConsumerWarps) {   // warp per row, lanes over columns
             const long long row_off = (tap_off + m0 + rr) * p.co;
             for (int c = 4 * lane; c < BN; c += 128) {
               const int co = n_tile * BN + c;
@@ -898,15 +566,11 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
             }
           }
         }
+        named_bar_sync(2, kConsumerThreads);               // s_last is rewritten by the next unit
       }
     }
   }
-  tc_fence_before();
-  if (CL > 1) cluster_sync_all(); else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
+  if (CL > 1) cluster_sync_all();                         // no CTA exits while its peer may still signal it
 }
 
 // dw = beta * dw + sum_s partial[s]   (fixed summation order => deterministic)
@@ -939,18 +603,16 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 static EncodeTiledFn g_encode = nullptr;
 static bool g_tma_store = true;     // RIGL_TMA_STORE=0 falls back to per-thread global stores
-static bool g_cta_pair = true;      // RIGL_CTA_PAIR=0: single-CTA MMA (M = 128) everywhere
-static bool g_pair_local = false;   // RIGL_PAIR_LOCALBAR=1: per-CTA full barriers + a forwarded arrive (measured 2.5x SLOWER than signalling the leader directly; kept as a documented negative result)
 // RIGL_WGRAD_FIXUP=1: the last-arriving CTA of an output tile sums the split-K partials inside the wgrad kernel
-// instead of a separate k_splitk_reduce launch.  MEASURED SLOWER on ResNet-50 b256 (wgrad 4.3 -> 10.7 ms per step):
-// the layers with few output tiles run 100-300 splits, and one CTA then sums 20 MB that the separate kernel
-// spreads over the whole grid.  Kept opt-in as a documented negative result.
+// instead of a separate k_splitk_reduce launch.  Off by default: the layers with few output tiles run 100-300
+// splits, and one CTA then sums tens of MB that the separate kernel spreads over the whole grid.
 static bool g_wgrad_fixup = false;
+// RIGL_CLUSTER_MC=1: 2-CTA clusters whose CTAs share the weight tile (fprop/dgrad) or the dY tile (wgrad): each loads
+// half of it and multicasts it to both, halving those L2 -> SM bytes.  Opt-in; the single-CTA kernels are the default.
+static bool g_cluster_mc = false;
 static bool g_bn_stats_always = false;   // RIGL_BN_STATS_ALWAYS=1: epilogue statistics for every supported shape (tests)
 static bool g_halo = true;          // RIGL_HALO3X3=0: 3x3/s1 layers with <= 64 channels use the generic kernels
 static int g_halo_t = 0, g_halo_nbuf = 0;   // RIGL_HALO_CFG=T,NBUF: tuning override for the halo kernels
-static bool g_cluster_mc = false;   // RIGL_CLUSTER_MC=1 enables the 2-CTA multicast clusters (measured neutral
-                                    // on ResNet-50 b256: the main loops are not L2-bandwidth bound)
 static int g_num_sms = 0;
 static std::once_flag g_once;
 static int g_init_status = RIGL_OK;
@@ -966,17 +628,15 @@ static void init_driver() {
   }
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   if (const char* e = getenv("RIGL_TMA_STORE")) g_tma_store = !(e[0] == '0');
-  if (const char* e = getenv("RIGL_CLUSTER_MC")) g_cluster_mc = (e[0] == '1');
-  if (const char* e = getenv("RIGL_CTA_PAIR")) g_cta_pair = !(e[0] == '0');
   if (const char* e = getenv("RIGL_HALO3X3")) g_halo = !(e[0] == '0');
   if (const char* e = getenv("RIGL_BN_STATS_ALWAYS")) g_bn_stats_always = (e[0] == '1');
   if (const char* e = getenv("RIGL_WGRAD_FIXUP")) g_wgrad_fixup = (e[0] == '1');
-  if (const char* e = getenv("RIGL_PAIR_LOCALBAR")) g_pair_local = (e[0] == '1');
+  if (const char* e = getenv("RIGL_CLUSTER_MC")) g_cluster_mc = (e[0] == '1');
   if (const char* e = getenv("RIGL_HALO_CFG")) sscanf(e, "%d,%d", &g_halo_t, &g_halo_nbuf);
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  if (g_num_sms <= 0) g_num_sms = 148;
+  if (g_num_sms <= 0) g_num_sms = kNumSmsHint;
 }
 
 static int ensure_driver() {
@@ -1044,7 +704,7 @@ static inline int posmod(int a, int b) { return ((a % b) + b) % b; }
 
 int tc_max_ctas() {
   ensure_driver();
-  return g_num_sms > 0 ? g_num_sms : 148;
+  return g_num_sms > 0 ? g_num_sms : kNumSmsHint;
 }
 
 bool tc_supported(const ConvGeom& g, int which) {
@@ -1060,7 +720,7 @@ static size_t wgrad_ws_elems(const ConvGeom& g, int* splits_out, int* bps_out, i
   const int tiles_w = (g.out_w + bw - 1) / bw, tiles_h = (g.out_h + bh - 1) / bh, tiles_n = (g.batch + bn - 1) / bn;
   const int pblocks = tiles_w * tiles_h * tiles_n;
   const int out_tiles = g.taps() * ((g.cin + kBM - 1) / kBM) * ((g.cout + bn_tile - 1) / bn_tile);
-  const int sms = g_num_sms > 0 ? g_num_sms : 148;
+  const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   int splits = (2 * sms + out_tiles - 1) / out_tiles;
   if (splits > pblocks) splits = pblocks;
   if (splits < 1) splits = 1;
@@ -1076,12 +736,9 @@ static size_t wgrad_counter_bytes(const ConvGeom& g, int bn_tile) {
   return (tiles * sizeof(int) + 255) / 256 * 256;
 }
 
-// Wider N tiles halve the L2->smem bytes per FLOP (the wgrad main loop is L2-bandwidth bound:
-// K blocks are only 64 pixels deep).
-static int wgrad_bn_tile(const ConvGeom& g) {
-  if (g.cout >= 256 && g.cin >= 256) return 256;      // (measured: narrow-Cin layers prefer more, smaller units)
-  return g.cout >= 128 ? 128 : 64;
-}
+// Wider N tiles halve the L2->smem bytes per FLOP (the wgrad main loop is L2-bandwidth bound: K blocks are
+// only 64 pixels deep); 128 is the widest whose accumulators fit the consumer warpgroups' registers.
+static int wgrad_bn_tile(const ConvGeom& g) { return g.cout >= 128 ? 128 : 64; }
 
 #include "halo3x3.cuh"
 #include "stem_s2d.cuh"
@@ -1096,19 +753,15 @@ size_t tc_workspace_bytes(const ConvGeom& g) {
   return elems * sizeof(float) + wgrad_counter_bytes(g, wgrad_bn_tile(g)) + 256;
 }
 
-// With the 2-CTA multicast each CTA fetches half of the weight tile (B box = bn_tile/2 rows).
-static bool kmajor_use_pair(const IgemmParams& p) {      // CTA-pair (cta_group::2) kernel
-  return g_cta_pair && p.tiles_w * p.tiles_h * p.tiles_n >= 2;
+static bool kmajor_use_mc(const IgemmParams& p) {      // multicast needs a partner M tile
+  return g_cluster_mc && p.tiles_w * p.tiles_h * p.tiles_n >= 2;
 }
-static bool kmajor_use_mc(const IgemmParams& p) {
-  return !kmajor_use_pair(p) && g_cluster_mc && p.tiles_w * p.tiles_h * p.tiles_n >= 2;
-}
-static int kmajor_b_rows(const IgemmParams& p, int bn_tile) {
-  return (kmajor_use_mc(p) || kmajor_use_pair(p)) ? bn_tile / 2 : bn_tile;
+static int kmajor_b_rows(const IgemmParams& p, int bn_tile) {   // with the multicast each CTA fetches half of B
+  return kmajor_use_mc(p) ? bn_tile / 2 : bn_tile;
 }
 
 static int kmajor_grid(const IgemmParams& p) {         // CTAs the K-major launcher will use (p.n_tiles set)
-  const int cl = (kmajor_use_mc(p) || kmajor_use_pair(p)) ? 2 : 1;
+  const int cl = kmajor_use_mc(p) ? 2 : 1;
   const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
   const int pairs = ((m_tiles + cl - 1) / cl) * p.n_tiles;
   int clusters = g_num_sms / cl;
@@ -1116,21 +769,15 @@ static int kmajor_grid(const IgemmParams& p) {         // CTAs the K-major launc
   return clusters * cl;
 }
 
-template <int BN, int STAGES, int CL>
-static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap, const IgemmParams& p,
-                         cudaStream_t s) {
-  constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 2 * (kBM * 64 * 2) + 1024 + 256;
-  static bool configured = false;
-  if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
+// Launch with a cluster of CL CTAs along x (CL == 1: a plain launch).
+template <int CL, typename Kern, typename... Args>
+static int launch_clustered(Kern kern, int grid, size_t smem, cudaStream_t s, Args... args) {
+  if (CL == 1) {
+    kern<<<(unsigned)grid, kThreads, smem, s>>>(args...);
+    return RIGL_OK;
   }
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int pairs = ((m_tiles + CL - 1) / CL) * p.n_tiles;
-  int clusters = g_num_sms / CL;
-  if (pairs < clusters) clusters = pairs;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(clusters * CL));
+  cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
@@ -1139,63 +786,39 @@ static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUt
   attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (CL == 1) {
-    k_igemm_kmajor<BN, STAGES, CL><<<cfg.gridDim, cfg.blockDim, smem, s>>>(amaps, bmap, omap, p);
-  } else {
-    RIGL_CUDA(cudaLaunchKernelEx(&cfg, k_igemm_kmajor<BN, STAGES, CL>, amaps, bmap, omap, p));
-  }
-  RIGL_LAUNCH_CHECK("k_igemm_kmajor");
+  RIGL_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
   return RIGL_OK;
 }
 
-template <int BN, int STAGES>
-static int launch_kmajor2(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap, const IgemmParams& p,
-                          cudaStream_t s) {
-  constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + (BN / 2) * kBK * 2) + 2 * (kBM * 64 * 2) + 1024 + 512;
+template <int BN, int STAGES, int CL>
+static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap, const IgemmParams& p,
+                         cudaStream_t s) {
+  constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 2 * (kBM * 64 * 2) + 1024 + 256;
+  static_assert(smem <= 227 * 1024, "K-major kernel exceeds the shared memory of an SM");
   static bool configured = false;
   if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor2<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int pairs = ((m_tiles + 1) / 2) * p.n_tiles;
-  int clusters = g_num_sms / 2;
-  if (pairs < clusters) clusters = pairs;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(clusters * 2));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  RIGL_CUDA(cudaLaunchKernelEx(&cfg, k_igemm_kmajor2<BN, STAGES>, amaps, bmap, omap, p));
-  RIGL_LAUNCH_CHECK("k_igemm_kmajor2");
+  const int rc = launch_clustered<CL>(k_igemm_kmajor<BN, STAGES, CL>, kmajor_grid(p), smem, s, amaps, bmap, omap, p);
+  if (rc != RIGL_OK) return rc;
+  RIGL_LAUNCH_CHECK("k_igemm_kmajor");
   return RIGL_OK;
 }
 
 static int dispatch_kmajor(int n_out, const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
                            IgemmParams& p, int bn_tile, cudaStream_t s) {
   p.n_tiles = (n_out + bn_tile - 1) / bn_tile;
-  if (kmajor_use_pair(p)) {               // CTA-pair MMA (M = 256); bmap was built with bn_tile/2 rows
-    p.pair_local = g_pair_local ? 1 : 0;
-    if (bn_tile == 64) return launch_kmajor2<64, 9>(amaps, bmap, omap, p, s);
-    if (bn_tile == 128) return launch_kmajor2<128, 8>(amaps, bmap, omap, p, s);
-    return launch_kmajor2<256, 6>(amaps, bmap, omap, p, s);
-  }
-  const bool mc = kmajor_use_mc(p);                        // multicast needs a partner M tile
-  if (bn_tile == 64) return mc ? launch_kmajor<64, 8, 2>(amaps, bmap, omap, p, s) : launch_kmajor<64, 8, 1>(amaps, bmap, omap, p, s);
-  if (bn_tile == 128) return mc ? launch_kmajor<128, 6, 2>(amaps, bmap, omap, p, s) : launch_kmajor<128, 6, 1>(amaps, bmap, omap, p, s);
-  return mc ? launch_kmajor<256, 4, 2>(amaps, bmap, omap, p, s) : launch_kmajor<256, 4, 1>(amaps, bmap, omap, p, s);
+  const bool mc = kmajor_use_mc(p);                        // bmap was built with kmajor_b_rows(p, bn_tile) rows
+  if (bn_tile == 64) return mc ? launch_kmajor<64, 7, 2>(amaps, bmap, omap, p, s) : launch_kmajor<64, 7, 1>(amaps, bmap, omap, p, s);
+  return mc ? launch_kmajor<128, 5, 2>(amaps, bmap, omap, p, s) : launch_kmajor<128, 5, 1>(amaps, bmap, omap, p, s);
 }
 
 static int pick_bn(int n_out, long long m_tiles) {
-  // Keep at least ~1 wave of CTAs busy; otherwise prefer the widest tile (fewest A re-reads).
-  if (n_out > 128 && m_tiles * ((n_out + 255) / 256) >= 148) return 256;
-  if (n_out > 64) return 128;
-  return 64;
+  // The widest tile whose accumulators fit the consumer warpgroups' registers (64 x 128 fp32 per warpgroup):
+  // fewest A re-reads.
+  (void)m_tiles;
+  return n_out > 64 ? 128 : 64;
 }
 
 void tc_set_bn_stats_always(bool on) { g_bn_stats_always = on; }
@@ -1220,10 +843,10 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
     }
   }
   if (bn_partial != nullptr && !g_bn_stats_always) {
-    // Measured on B200 (ResNet-50 b256, profiles/r02_bn_stats_epilogue.md): the statistics are free when the tile's
-    // main loop is long enough to hide them (reduction length K = taps * cin >= 512), and cost about what the
-    // separate stats pass costs -- or more -- for the short-K / wide-output layers whose epilogue is the
-    // bottleneck (1x1 convs with K <= 128; K = 256 with more than 128 output channels).
+    // The statistics are free when the tile's main loop is long enough to hide them (reduction length
+    // K = taps * cin >= 512), and cost about what the separate stats pass costs -- or more -- for the short-K /
+    // wide-output layers whose epilogue is the bottleneck (1x1 convs with K <= 128; K = 256 with more than 128
+    // output channels).
     const int K = g.taps() * g.cin;
     if (!(K >= 512 || (K >= 256 && g.cout <= 128))) {
       set_error("fused BN statistics: not profitable for this shape (K = %d, cout = %d)", K, g.cout);
@@ -1361,30 +984,17 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
 template <int BN, int STAGES, int CL>
 static int launch_wgrad_cl(const TMaps4& xmaps, const CUtensorMap& dymap, const WgradParams& p, cudaStream_t s) {
   constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 1024 + 256;
+  static_assert(smem <= 227 * 1024, "wgrad kernel exceeds the shared memory of an SM");
   static bool configured = false;
   if (!configured) {
     RIGL_CUDA(cudaFuncSetAttribute(k_igemm_wgrad<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  const int mcount = p.ntaps * p.m_tiles;
-  const int groups = ((mcount + CL - 1) / CL) * p.n_tiles * p.splits;
+  const int groups = ((p.ntaps * p.m_tiles + CL - 1) / CL) * p.n_tiles * p.splits;
   int clusters = g_num_sms / CL;
   if (groups < clusters) clusters = groups;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(clusters * CL));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (CL == 1) {
-    k_igemm_wgrad<BN, STAGES, CL><<<cfg.gridDim, cfg.blockDim, smem, s>>>(xmaps, dymap, p);
-  } else {
-    RIGL_CUDA(cudaLaunchKernelEx(&cfg, k_igemm_wgrad<BN, STAGES, CL>, xmaps, dymap, p));
-  }
+  const int rc = launch_clustered<CL>(k_igemm_wgrad<BN, STAGES, CL>, clusters * CL, smem, s, xmaps, dymap, p);
+  if (rc != RIGL_OK) return rc;
   RIGL_LAUNCH_CHECK("k_igemm_wgrad");
   return RIGL_OK;
 }
@@ -1467,9 +1077,7 @@ int tc_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float 
   CUtensorMap dymap;
   rc = make_act_map(&dymap, dy, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, box);
   if (rc != RIGL_OK) return rc;
-  rc = (bn_tile == 256)   ? launch_wgrad<256, 4>(xmaps, dymap, p, s)
-       : (bn_tile == 128) ? launch_wgrad<128, 6>(xmaps, dymap, p, s)
-                          : launch_wgrad<64, 8>(xmaps, dymap, p, s);
+  rc = (bn_tile == 128) ? launch_wgrad<128, 6>(xmaps, dymap, p, s) : launch_wgrad<64, 8>(xmaps, dymap, p, s);
   if (rc != RIGL_OK) return rc;
   if (!direct && p.counters == nullptr) {
     const long long threads = (n_w + 3) / 4;
@@ -1560,7 +1168,7 @@ size_t smallc_packed_bytes(const ConvGeom& g) { return (size_t)g.ksize * g.cout 
 
 int smallc_pad_input(const ConvGeom& g, const void* x, void* xp, cudaStream_t s) {
   const SmallCGeom q = smallc_geom(g);
-  k_smallc_pad<<<148 * 16, 256, 0, s>>>(g, q.hp, q.wp, (const __nv_bfloat16*)x, (__nv_bfloat16*)xp);
+  k_smallc_pad<<<kNumSmsHint * 16, 256, 0, s>>>(g, q.hp, q.wp, (const __nv_bfloat16*)x, (__nv_bfloat16*)xp);
   RIGL_LAUNCH_CHECK("k_smallc_pad");
   return RIGL_OK;
 }
@@ -1678,9 +1286,7 @@ int smallc_wgrad(const ConvGeom& g, const void* xp, const void* dy, float* dw, f
   CUtensorMap dymap;
   rc = make_act_map(&dymap, dy, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, box);
   if (rc != RIGL_OK) return rc;
-  rc = (bn_tile == 256)   ? launch_wgrad<256, 4>(xmaps, dymap, p, s)
-       : (bn_tile == 128) ? launch_wgrad<128, 6>(xmaps, dymap, p, s)
-                          : launch_wgrad<64, 8>(xmaps, dymap, p, s);
+  rc = (bn_tile == 128) ? launch_wgrad<128, 6>(xmaps, dymap, p, s) : launch_wgrad<64, 8>(xmaps, dymap, p, s);
   if (rc != RIGL_OK) return rc;
   const long long total = (long long)g.ksize * g.ksize * g.cin * g.cout;
   k_smallc_unpack<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(g, p.out, p.split_stride, p.splits, dw, beta);

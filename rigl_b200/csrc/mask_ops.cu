@@ -91,7 +91,7 @@ extern "C" int rigl_mask_popcount(const uint32_t* bits, int64_t n, int32_t* out_
   const int64_t words = rigl_mask_words(n);
   RIGL_CUDA(cudaMemsetAsync(out_count_dev, 0, sizeof(int32_t), (cudaStream_t)stream));
   int blocks = (int)((words + 255) / 256);
-  if (blocks > 592) blocks = 592;
+  if (blocks > kNumSmsHint * 4) blocks = kNumSmsHint * 4;
   k_popcount<<<blocks, 256, 0, (cudaStream_t)stream>>>(bits, words, out_count_dev);
   RIGL_LAUNCH_CHECK("k_popcount");
   return RIGL_OK;

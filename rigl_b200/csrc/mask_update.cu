@@ -1,4 +1,4 @@
-// Batched RigL/SET mask update on sm_100a: exact top-k drop by |mask*w| (+noise)
+// Batched RigL/SET mask update on sm_90a: exact top-k drop by |mask*w| (+noise)
 // and exact top-k grow by |dense grad| with tf.nn.top_k tie semantics
 // (equal scores -> lower flat index first), for ALL masked layers of a model in
 // one 7-node launch sequence, masks stored as 1-bit bitmaps.

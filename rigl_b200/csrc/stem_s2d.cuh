@@ -1,24 +1,21 @@
-// Space-to-depth stem kernels (layers.STEM_S2D_PATH, default on; validated on B200 in round 2 by
-// tools/umma_sw32_probe.cu and tests/test_conv_gpu.py::test_conv_stem_s2d_path).  Design: DESIGN.md 3.7.
+// Space-to-depth stem kernels (layers.STEM_S2D_PATH, default on; tests/test_conv_gpu.py::test_conv_stem_s2d_path).
+// Design: DESIGN.md 3.2.
 //
 // The 7x7 / stride-2 / 3-channel stem without a patch matrix.  The zero-padded input is folded
 // 2x2 -> channels ("space to depth"): xs[n, hs, ws, (dy*2+dx)*3 + c] = xpad[n, 2hs+dy, 2ws+dx, c],
 // 16 bf16 = 32 bytes per folded pixel (slots 12..15 zero).  The conv becomes a 4x4 / stride-1
 // conv over 16 channels (taps (th, tw), weights of the non-existent kh = 7 / kw = 7 zero), i.e.
-// exactly ONE K = 16 tcgen05.mma per tap, and the halo trick of halo3x3.cuh applies with
-// 32-byte rows: one halo tile of (R+3) folded rows x 128 columns (TMA, SWIZZLE_32B, OOB zero fill)
-// feeds all 16 taps through row-shifted descriptors (tap (th,tw): +th*128 + tw rows).  An M tile
-// is one output row (128 positions, 112 valid); the 32 KB weight operand stays resident.
+// exactly ONE K = 16 wgmma per tap, and the halo trick of halo3x3.cuh applies with 32-byte rows:
+// one halo tile of (R+3) folded rows x 128 columns (TMA, SWIZZLE_32B, OOB zero fill) feeds all 16
+// taps; the A fragment of tap (th, tw) starts th*128 + tw rows down the tile and is loaded with
+// ldmatrix at explicitly swizzled addresses.  An M tile is one output row (128 positions, 112 valid);
+// the 32 KB weight operand stays resident.
 //
-// wgrad: A = the same halo tile read MN-major (row = position = K index, 32 B = 16 folded channels):
-// M = 128 is EIGHT 16-channel atoms LBO = 32 B apart = eight horizontally neighbouring taps
-// (tw = 0..7, the last four unused), so one MMA per th accumulates a whole filter row; B = the dY
-// tile (MN-major, SWIZZLE_128B, padding columns zero-filled by TMA).  Four accumulators of 64
-// columns; per-CTA fp32 partials [th][tw*16 + k16][co], then k_stem_s2d_reduce scatters them into
-// the dense HWIO gradient in CTA order (deterministic).
-//
-// Open hardware questions (tools/umma_sw32_probe.cu): row-shifted descriptors under SWIZZLE_32B,
-// and 8 MN atoms addressed through LBO.
+// wgrad: for filter row th, D_th[tw*16 + k16][co] = sum_q xs_tile[q + th*128 + tw][k16] * dY[q][co] over the
+// four horizontal taps tw = 0..3: M = 64, one wgmma per (th, 16 positions), A = the shifted tile read transposed
+// (ldmatrix.trans), B = the dY tile (MN-major, SWIZZLE_128B, padding columns zero-filled by TMA).  Per-CTA fp32
+// partials [th][tw*16 + k16][co] (rows 64..127 of each th block unused), then k_stem_s2d_reduce scatters them
+// into the dense HWIO gradient in CTA order (deterministic).
 //
 // Included by igemm_tc.cu inside namespace rigl.
 #pragma once
@@ -38,17 +35,6 @@ struct S2dParams {
 
 constexpr int kS2dWp = 128;                               // halo pitch (positions per M tile)
 constexpr uint32_t kS2dBTapBytes = 64 * 16 * 2;           // one tap of the weight operand: 64 rows x 32 B
-constexpr uint32_t kS2dSwz32 = 6;                         // UMMA descriptor layout type: SWIZZLE_32B
-
-__device__ __forceinline__ uint64_t make_smem_desc_swz(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swz) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)swz << 61;
-  return d;
-}
 
 // ---- input fold: x [N,H,W,cin<=3] (pitch x_pitch) -> xs [N,HS,WS,16] ----
 __global__ void __launch_bounds__(256)
@@ -98,7 +84,6 @@ __global__ void __launch_bounds__(kThreads, 1)
 k_stem_s2d_fprop(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
                  const __grid_constant__ CUtensorMap omap, const S2dParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr uint32_t kIdesc = make_idesc_bf16(128, 64, 0, 0);
   constexpr uint32_t kSlab = 128 * 64 * 2;
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t b_base = smem_base;                                   // 16 taps x 2 KB
@@ -108,24 +93,15 @@ k_stem_s2d_fprop(const __grid_constant__ CUtensorMap amap, const __grid_constant
   const uint32_t b_full = bar_base;
   auto a_full = [&](int b) { return bar_base + 8u * (1 + b); };
   auto a_empty = [&](int b) { return bar_base + 8u * (5 + b); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (9 + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (11 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * 13;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&amap); prefetch_tmap(&bmap); prefetch_tmap(&omap);
     mbar_init(b_full, 1);
-    for (int b = 0; b < p.nbuf; ++b) { mbar_init(a_full(b), 1); mbar_init(a_empty(b), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
+    for (int b = 0; b < p.nbuf; ++b) { mbar_init(a_full(b), 1); mbar_init(a_empty(b), kConsumerWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   if (warp == 0) {
     if (elect_one()) {
@@ -141,117 +117,78 @@ k_stem_s2d_fprop(const __grid_constant__ CUtensorMap amap, const __grid_constant
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
+  } else if (warp >= kConsumerWarp0) {
+    const int cw = warp - kConsumerWarp0;
+    const int wg = cw >> 2;
+    const int row = 64 * wg + 16 * (cw & 3) + (lane >> 2);
+    const int lrow = 64 * wg + 16 * (cw & 3) + (lane & 7) + 8 * ((lane >> 3) & 1);
+    const uint32_t lk = (uint32_t)(lane >> 4) * 16u;
+    const bool issuer = (cw == 0 && lane == 0);
+    const uint64_t b_desc0 = make_smem_desc(b_base, 16, 256, kSwz32);
     mbar_wait(b_full, 0);
     int buf = 0; uint32_t phase = 0;
-    int acc = 0; uint32_t acc_phase = 0;
-    const uint64_t b_desc0 = make_smem_desc_swz(b_base, 16, 256, kS2dSwz32);
-    for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
-      mbar_wait(a_full(buf), phase);
-      tc_fence_after();
-      const uint64_t a_desc0 = make_smem_desc_swz(a_base + buf * p.a_buf_bytes, 16, 256, kS2dSwz32);
-      for (int t = 0; t < p.R; ++t) {                        // M tile t = output row h0 + t
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 64);
-        if (elect_one()) {
-#pragma unroll
-          for (int tap = 0; tap < 16; ++tap) {               // rows of 32 B = 2 address units each
-            const int row = (t + (tap >> 2)) * kS2dWp + (tap & 3);
-            umma_bf16(d_tmem, a_desc0 + (uint64_t)(row * 2), b_desc0 + (uint64_t)(tap * (kS2dBTapBytes >> 4)), kIdesc,
-                      tap == 0 ? 0u : 1u);
-          }
-          umma_commit(tfull_bar(acc));
-        }
-        __syncwarp();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-      if (elect_one()) umma_commit(a_empty(buf));
-      __syncwarp();
-      if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
-    }
-  } else {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const bool issuer = (warp == 2 && lane == 0);
-    int acc = 0; uint32_t acc_phase = 0;
     uint32_t slab_ctr = 0;
     for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
       const int n = strip / p.strips_per_image, h0 = (strip % p.strips_per_image) * p.R;
-      for (int t = 0; t < p.R; ++t) {
-        mbar_wait(tfull_bar(acc), acc_phase);
-        tc_fence_after();
+      mbar_wait(a_full(buf), phase);
+      const uint32_t a_tile = a_base + buf * p.a_buf_bytes;
+      for (int t = 0; t < p.R; ++t) {                        // M tile t = output row h0 + t
+        float acc[32];
+        zero_acc(acc);
+        uint32_t a[2][4];
+#pragma unroll
+        for (int tap = 0; tap < 16; ++tap) {                 // rows of 32 B
+          const int r = (t + (tap >> 2)) * kS2dWp + (tap & 3) + lrow;
+          ldmatrix_x4(a[tap & 1], swz32(a_tile + (uint32_t)r * 32u + lk));
+          fence_regs(acc);
+          wgmma_fence();
+          Wgmma<64>::rs<0>(acc, a[tap & 1], b_desc0 + (uint64_t)(tap * (kS2dBTapBytes >> 4)));
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (tap > 0) keep_frag(a[(tap + 1) & 1]);
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        keep_frag(a[1]);
         const uint32_t slab = out_base + (slab_ctr & 1u) * kSlab;
         if (issuer) tma_store_wait_read<1>();
-        named_bar_sync(1, 128);
-        uint32_t r0[32], r1[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * 64), r0);
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * 64 + 32), r1);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(acc));
-        const uint32_t row_addr = slab + (uint32_t)row * 128u;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          uint32_t pk[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int e = 8 * j + 2 * q;
-            const float a = __uint_as_float(e < 32 ? r0[e] : r1[e - 32]);
-            const float b = __uint_as_float(e + 1 < 32 ? r0[e + 1] : r1[e + 1 - 32]);
-            __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-            pk[q] = *reinterpret_cast<uint32_t*>(&h);
-          }
-          const uint32_t dst = row_addr + (uint32_t)((j ^ (row & 7)) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]),
-                       "r"(pk[3])
-                       : "memory");
-        }
+        named_bar_sync(1, kConsumerThreads);
+        stage_slab<0>(acc, slab, row, true, true, lane);     // columns >= W and rows >= H are clipped by the store
         fence_proxy_async_smem();
-        named_bar_sync(1, 128);
-        if (issuer) {                                        // columns >= W and rows >= H are clipped by TMA
+        named_bar_sync(1, kConsumerThreads);
+        if (issuer) {
           tma_store_4d(&omap, slab, 0, 0, h0 + t, n);
           tma_store_commit();
         }
         ++slab_ctr;
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(a_empty(buf));
+      if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
     }
     if (issuer) tma_store_wait_all();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
   }
 }
 
 // ---- wgrad ----
+// Consumer warpgroup wg accumulates filter rows th = 2wg, 2wg + 1; warp w of it owns the rows tw = w of both.
 __global__ void __launch_bounds__(kThreads, 1)
 k_stem_s2d_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant__ CUtensorMap dymap,
                  const S2dParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  constexpr uint32_t kIdesc = make_idesc_bf16(128, 64, 1, 1);
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t dy_bytes = (uint32_t)(p.R * kS2dWp) * 128u;
   const uint32_t stage_bytes = p.a_buf_bytes + dy_bytes;               // [x halo | dy]
   const uint32_t bar_base = smem_base + p.nbuf * stage_bytes;
   auto full_bar = [&](int b) { return bar_base + 8u * b; };
   auto empty_bar = [&](int b) { return bar_base + 8u * (4 + b); };
-  const uint32_t tfull = bar_base + 8u * 8;
-  const uint32_t tmem_slot = bar_base + 8u * 9;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&xmap); prefetch_tmap(&dymap);
-    for (int b = 0; b < p.nbuf; ++b) { mbar_init(full_bar(b), 1); mbar_init(empty_bar(b), 1); }
-    mbar_init(tfull, 1);
+    for (int b = 0; b < p.nbuf; ++b) { mbar_init(full_bar(b), 1); mbar_init(empty_bar(b), kConsumerWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
   {   // slack rows behind each halo tile are read against zero dY columns: they must be finite
     const uint32_t slack = p.a_buf_bytes - p.a_tx_bytes;
     for (int b = 0; b < p.nbuf; ++b)
@@ -260,10 +197,7 @@ k_stem_s2d_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant
                      : "memory");
     fence_proxy_async_smem();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   if (warp == 0) {
     if (elect_one()) {
@@ -279,61 +213,57 @@ k_stem_s2d_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
+  } else if (warp >= kConsumerWarp0) {
+    const int cw = warp - kConsumerWarp0;
+    const int wg = cw >> 2, tw = cw & 3;
+    // ldmatrix.trans: lane supplies position (K) row 8 * (lane >> 4) + (lane & 7) of matrix lane / 8, whose 8
+    // folded channels are the 16-byte half (lane >> 3) & 1 of the 32-byte row.
+    const uint32_t lpos = (uint32_t)(8 * (lane >> 4) + (lane & 7));
+    const uint32_t lhalf = (uint32_t)((lane >> 3) & 1) * 16u;
+    float acc[2][32];
+    zero_acc(acc[0]); zero_acc(acc[1]);
+    uint32_t a[2][4];
     int buf = 0; uint32_t phase = 0;
-    bool first = true;
     const int ksteps = p.R * kS2dWp / 16;
     for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
       mbar_wait(full_bar(buf), phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t x_src = smem_base + buf * stage_bytes;
-        const uint64_t db0 = make_smem_desc_swz(x_src + p.a_buf_bytes, 8192, 1024, 2);          // dY: 128-byte rows
-        uint64_t da0[4];
+      const uint32_t x_src = smem_base + buf * stage_bytes;
+      const uint64_t db0 = make_smem_desc(x_src + p.a_buf_bytes, 8192, 1024);     // dY: 128-byte rows
+#pragma unroll 1
+      for (int k = 0; k < ksteps; ++k) {                   // 16 positions: +512 B of x rows, +2048 B of dY rows
 #pragma unroll
-        for (int th = 0; th < 4; ++th)       // 8 atoms of 16 channels, one 32-byte row apart: taps (th, tw = 0..7)
-          da0[th] = make_smem_desc_swz(x_src + (uint32_t)(th * kS2dWp) * 32u, 32, 256, kS2dSwz32);
-#pragma unroll 2
-        for (int k = 0; k < ksteps; ++k) {                   // 16 positions: +512 B of x rows, +2048 B of dY rows
-#pragma unroll
-          for (int th = 0; th < 4; ++th)
-            umma_bf16(tmem_base + (uint32_t)(th * 64), da0[th] + (uint64_t)(32 * k), db0 + (uint64_t)(128 * k), kIdesc,
-                      (first && k == 0) ? 0u : 1u);
+        for (int i = 0; i < 2; ++i) {
+          const int th = 2 * wg + i;
+          const uint32_t r = (uint32_t)(16 * k + th * kS2dWp + tw) + lpos;
+          ldmatrix_x4_trans(a[i], swz32(x_src + r * 32u + lhalf));
+          fence_regs(acc[i]);
+          wgmma_fence();
+          Wgmma<64>::rs<1>(acc[i], a[i], db0 + (uint64_t)(128 * k));
+          wgmma_commit();
+          wgmma_wait<1>();                                 // the MMA that last read a[i ^ 1] has retired
+          keep_frag(a[i ^ 1]);
         }
-        umma_commit(empty_bar(buf));
       }
+      wgmma_wait<0>();
+      fence_regs(acc[0]); fence_regs(acc[1]);
+      keep_frag(a[0]); keep_frag(a[1]);
       __syncwarp();
-      first = false;
+      if (lane == 0) mbar_arrive(empty_bar(buf));
       if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
     }
-    if (elect_one()) umma_commit(tfull);
-    __syncwarp();
-  } else {
-    const int quad = warp & 3;
-    mbar_wait(tfull, 0);
-    tc_fence_after();
     float* part = p.wgrad_out + (size_t)blockIdx.x * 4 * 128 * 64;
-#pragma unroll 1
-    for (int th = 0; th < 4; ++th) {
-      float* dst_row = part + ((size_t)th * 128 + quad * 32 + lane) * 64;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t r32[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(th * 64 + c0), r32);
-        tmem_ld_wait();
 #pragma unroll
-        for (int q = 0; q < 32; q += 4)
-          *reinterpret_cast<float4*>(dst_row + c0 + q) =
-              make_float4(__uint_as_float(r32[q]), __uint_as_float(r32[q + 1]), __uint_as_float(r32[q + 2]),
-                          __uint_as_float(r32[q + 3]));
+    for (int i = 0; i < 2; ++i) {
+      const int th = 2 * wg + i;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float* dst_row = part + ((size_t)th * 128 + tw * 16 + (lane >> 2) + 8 * h) * 64;
+#pragma unroll
+        for (int jc = 0; jc < 8; ++jc)
+          *reinterpret_cast<float2*>(dst_row + 8 * jc + 2 * (lane & 3)) =
+              make_float2(acc[i][4 * jc + 2 * h], acc[i][4 * jc + 2 * h + 1]);
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -382,7 +312,7 @@ size_t s2d_folded_bytes(const ConvGeom& g) {
 size_t s2d_packed_bytes(const ConvGeom& g) { return (size_t)16 * g.cout * 32; }
 static int s2d_wgrad_grid(const S2dParams& p) {
   ensure_driver();
-  const int sms = g_num_sms > 0 ? g_num_sms : 148;
+  const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   return p.total_strips < sms ? p.total_strips : sms;
 }
 size_t s2d_workspace_bytes(const ConvGeom& g) {
@@ -394,7 +324,7 @@ size_t s2d_workspace_bytes(const ConvGeom& g) {
 int s2d_fold(const ConvGeom& g, const void* x, void* xs, cudaStream_t s) {
   S2dParams p;
   if (!s2d_geom(g, &p, false)) { set_error("rigl_stem_s2d: unsupported geometry"); return RIGL_ERR_UNSUPPORTED; }
-  k_stem_s2d_fold<<<148 * 16, 256, 0, s>>>(g, p.HS, p.WS, (const __nv_bfloat16*)x, (__nv_bfloat16*)xs);
+  k_stem_s2d_fold<<<kNumSmsHint * 16, 256, 0, s>>>(g, p.HS, p.WS, (const __nv_bfloat16*)x, (__nv_bfloat16*)xs);
   RIGL_LAUNCH_CHECK("k_stem_s2d_fold");
   return RIGL_OK;
 }
@@ -436,7 +366,7 @@ int s2d_fprop(const ConvGeom& g, const void* xs, const void* packed, void* y, cu
     RIGL_CUDA(cudaFuncSetAttribute(k_stem_s2d_fprop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = smem;
   }
-  const int sms = g_num_sms > 0 ? g_num_sms : 148;
+  const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   const int grid = p.total_strips < sms ? p.total_strips : sms;
   k_stem_s2d_fprop<<<grid, kThreads, smem, s>>>(amap, bmap, omap, p);
   RIGL_LAUNCH_CHECK("k_stem_s2d_fprop");

@@ -41,9 +41,8 @@ def _bn_partial_rows():
 
 
 STEM_WINDOW_PATH = False     # route small-Cin convs through the window-tensor-map kernels
-# space-to-depth halo kernels for the 7x7/2 3-channel stem (csrc/stem_s2d.cuh, DESIGN.md 3.7): validated on
-# B200 at the start of round 2 (tools/umma_sw32_probe.cu + tests/test_conv_gpu.py::test_conv_stem_s2d_path);
-# RIGL_STEM_S2D=0 falls back to the patch-matrix (im2col) stem
+# space-to-depth halo kernels for the 7x7/2 3-channel stem (csrc/stem_s2d.cuh, DESIGN.md 3.2; checked by
+# tests/test_conv_gpu.py::test_conv_stem_s2d_path); RIGL_STEM_S2D=0 falls back to the patch-matrix (im2col) stem
 STEM_S2D_PATH = _os.environ.get('RIGL_STEM_S2D', '1') != '0'
 
 

@@ -268,9 +268,8 @@ class TrainHarness(object):
     self.dp = data_parallel
     # Gradient exchange under data parallelism.  Default: ONE all-reduce of the flat buffer between the two graph
     # replays (backward; optimizer).  RIGL_DP_OVERLAP=1: bucketed all-reduces launched from inside backward on a
-    # communication stream and captured with the step.  Measured on 8 x B200 (profiles/r02_bench_n8*.json): 22.12 vs
-    # 22.21 ms per step (N = 1: 21.6) -- the 102 MB exchange takes ~0.4 ms over NVSwitch, and hiding it costs as
-    # much in SM contention as it saves, so the simpler form is the default.
+    # communication stream and captured with the step.  The exchange is short against a step and hiding it costs SM
+    # time beside the persistent one-CTA-per-SM conv kernels, so the simpler form is the default.
     self._dp_overlap = os.environ.get('RIGL_DP_OVERLAP', '0') == '1'
     self._pack_ahead = on_cuda and os.environ.get('RIGL_PACK_AHEAD', '1') != '0'
     if self.dp is not None:
@@ -457,8 +456,8 @@ class _DepthwiseFn(torch.autograd.Function):
 class DepthwiseConv2d(nn.Module):
   """depthwise_conv2d_fixed_padding(kernel_size=3) of the reference's MobileNet-v1 (mobilenetv1_model.py:120-153):
   dense (un-masked), fp32 master weights in the torch depthwise layout [C,1,3,3], bf16 compute on the streaming
-  kernels of csrc/depthwise.cu when RIGL_NATIVE_DEPTHWISE=1; default: the stock cuDNN grouped conv, which was
-  the faster of the two on B200 when measured (DESIGN.md 3.4)."""
+  kernels of csrc/depthwise.cu when RIGL_NATIVE_DEPTHWISE=1; default: the stock cuDNN grouped conv (DESIGN.md
+  3.4)."""
 
   def __init__(self, channels, stride=1, device='cuda'):
     super(DepthwiseConv2d, self).__init__()

@@ -169,8 +169,8 @@ def test_maxpool_same_forward_backward(shape):
 
 
 # (n, h, w, cin, cout, k, stride, epilogue statistics expected): the halo kernels (3x3/s1, <= 64 channels) and the
-# space-to-depth stem have no statistics epilogue and fall back to the stats pass; the rest covers the CTA-pair and
-# single-CTA kernels, several N tiles (cout 512 / 1024), pixel grids that do not fill their boxes (7x7, 13x9) and
+# space-to-depth stem have no statistics epilogue and fall back to the stats pass; the rest covers the K-major
+# kernel with both tile widths, several N tiles (cout 512 / 1024), pixel grids that do not fill their boxes (7x7, 13x9) and
 # problems with many tiles per CTA.
 @pytest.mark.parametrize('case', [(4, 56, 56, 64, 64, 3, 1, None), (4, 16, 16, 64, 128, 3, 1, True), (2, 28, 28, 128, 256, 1, 1, True),
                                   (8, 14, 14, 64, 64, 3, 2, True), (3, 32, 32, 3, 64, 7, 2, False),

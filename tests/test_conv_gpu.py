@@ -233,21 +233,8 @@ def test_conv_halo_disabled_matches(case):
   assert 'GEN_OK' in out.stdout, out.stdout[-1500:]
 
 
-@pytest.mark.parametrize('case', [CONV_CASES[0], CONV_CASES[5], CONV_CASES[7], CONV_CASES[9], CONV_CASES[12]])
-def test_conv_single_cta_mma_path(case):
-  """The default K-major kernel is the CTA-pair one (cta_group::2); this keeps the single-CTA
-  (M = 128) kernel covered."""
-  import os, subprocess, sys
-  code = ('import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_conv_gpu as t; '
-          't._conv_case(%r, False); print("ONE_OK")' % (os.path.dirname(os.path.dirname(__file__)),
-                                                        os.path.dirname(__file__), case))
-  env = dict(os.environ, RIGL_CTA_PAIR='0')
-  out = subprocess.run([sys.executable, '-c', code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-  assert 'ONE_OK' in out.stdout, out.stdout[-1500:]
-
-
 # ---- BASELINE-size problems (C2: ResNet-50, batch 256, 224x224): many more tiles than CTAs, so the persistent
-# loops' TMEM double buffering, smem-ring wrap and split-K schedules run for many tiles per CTA.
+# tile loops, smem-ring wrap and split-K schedules run for many tiles per CTA.
 def _r50_erk80_sparsity():
   layers = orc.resnet50_masked_layers()
   sp = orc.get_sparsities([orc.FakeMask(n + '/mask:0', sh) for n, sh, _, _ in layers], 'erdos_renyi_kernel', 0.8, {})
@@ -298,7 +285,7 @@ def _run_both(layer, x, dy, force_simt):
 
 @pytest.mark.parametrize('case', _r50_b256_shapes(), ids=lambda c: 'h%d_c%d_%d_k%d_s%d' % (c[1], c[3], c[4], c[5], c[6]))
 def test_conv_b256_every_r50_shape_tensor_core_vs_cuda_core(case):
-  """Every distinct ResNet-50 conv shape at batch 256: the tcgen05 kernels against the shape-agnostic CUDA-core
+  """Every distinct ResNet-50 conv shape at batch 256: the tensor-core kernels against the shape-agnostic CUDA-core
   kernels on the SAME device inputs and packed operands (fp32 accumulation on both sides; bf16 outputs may differ
   by one rounding)."""
   n, h, w, cin, cout, k, stride, sparsity = case

@@ -2,8 +2,8 @@
 oracle's direct convolution: the 2x2 input fold, the [16 taps][cout][16] weight operand, the tap ->
 halo-row offsets and the partial -> HWIO scatter of the wgrad reduce are restated here in numpy
 exactly as rigl_b200/csrc/stem_s2d.cuh indexes them (k_stem_s2d_fold / _pack / _fprop / _wgrad /
-_reduce).  This pins the MATH of that path; the hardware layout questions (SWIZZLE_32B row shifts,
-8-atom MN-major operands) are what tools/umma_sw32_probe.cu is for."""
+_reduce).  This pins the MATH of that path; the hardware layout (SWIZZLE_32B tiles, row-shifted ldmatrix
+loads) is checked on the device by tests/test_conv_gpu.py::test_conv_stem_s2d_path."""
 import numpy as np
 import pytest
 

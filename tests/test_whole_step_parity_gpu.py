@@ -9,8 +9,8 @@ What is compared and how tight it can be (DESIGN.md 5, "whole-step bound"):
     gradient rounded to bf16 at the same points, fp32 arithmetic inside each op.  Against the plain fp32 oracle
     a whole-network comparison is meaningless at initialisation: a batch-normalised ReLU network amplifies any
     perturbation ~1.2x per layer, so bf16 storage alone moves the dense gradients of ResNet-50 by a relative L2
-    of ~1.3 -- measured on the CPU with no kernel involved (tools/noise_growth.py ->
-    profiles/r02_whole_step_noise_growth.md), and the CUDA step shows the same figures.
+    of ~1.3 -- measured on the CPU with no kernel involved (tools/noise_growth.py), and the CUDA step shows the
+    same figures.
   * With matching rounding points what remains is fp32 summation order plus the rare bf16 rounding flips it
     causes (~1e-4 of a tensor per rounding point), amplified the same way.  Two checks follow from that:
     (1) TEACHER-FORCED: every masked layer replayed alone on the oracle's tensors of this very step -- no
@@ -90,10 +90,9 @@ def _teacher_forced_layers(model, net, tol_act=1e-3, tol_dense=2e-5):
   train step: its stored (bf16) input activation x and the stored (bf16) gradient dy of its output.  Independent
   of how the network amplifies perturbations, so the bounds are tight:
     fprop / dgrad (bf16 outputs): relative L2 <= 1e-3 -- the two sides round fp32 accumulators that differ in
-      summation order, so a small fraction of elements lands on the neighbouring bf16 value
-      (measured on B200: <= 6.4e-5 fprop, <= 1.7e-4 dgrad over all layers of the three models);
+      summation order, so a small fraction of elements lands on the neighbouring bf16 value;
     DENSE wgrad (fp32 accumulators, identical bf16 operands): relative L2 <= 2e-5, the north-star's 1e-5-class
-      bound (measured: <= 7.8e-7 ResNet-50, 2.6e-6 WRN-22-2, 6.4e-7 MobileNet-v1)."""
+      bound."""
   out = {}
   for l in model.registry.layers():
     x, y, stride, padding = net.record[l.scope]

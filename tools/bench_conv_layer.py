@@ -1,7 +1,7 @@
 """Per-layer micro-benchmark of the masked conv kernels (fprop / dgrad / dense wgrad) through the
 same host calls the training step makes.  One JSON line per (shape, op): microseconds (CUDA
 events, median of --iters, inputs rotated through buffers larger than L2), dense-executed TFLOP/s
-and algorithmic GB/s.  Kernel-selection switches (RIGL_HALO3X3, RIGL_HALO_CFG, RIGL_CTA_PAIR ...)
+and algorithmic GB/s.  Kernel-selection switches (RIGL_HALO3X3, RIGL_HALO_CFG, RIGL_TMA_STORE ...)
 are read once per process: run one process per configuration.
 
   python tools/bench_conv_layer.py [--shapes r50s1] [--iters 20] [--tag name]

@@ -1,4 +1,4 @@
-"""On-device cross-check of the tcgen05 implicit-GEMM kernels against the CUDA-core
+"""On-device cross-check of the tensor-core (wgmma) implicit-GEMM kernels against the CUDA-core
 kernels (same packed operands, same inputs), case by case, never stopping at a
 failure.  Prints one line per (case, op) with max abs error / scale.
 
