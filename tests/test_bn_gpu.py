@@ -8,6 +8,8 @@ import torch
 
 from rigl_b200.norm import FusedBatchNormReLU
 
+from isolated import assert_not_ran, assert_ran, run_isolated
+
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
 
@@ -76,13 +78,10 @@ def test_bn_forward_backward(shape, relu, residual):
 def test_bn_three_kernel_path(shape):
   """Small tensors take the single-launch (grid-barrier) kernels by default; RIGL_BN_FUSED=0 keeps the
   3-kernel path (the only one large tensors use) covered at oracle-checkable sizes."""
-  import os, subprocess, sys
-  code = ('import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_bn_gpu as t; '
-          '[t.test_bn_forward_backward(%r, relu, res) for relu, res in ((True, False), (False, False), (True, True))]; '
-          'print("BN3_OK")' % (os.path.dirname(os.path.dirname(__file__)), os.path.dirname(__file__), shape))
-  env = dict(os.environ, RIGL_BN_FUSED='0')
-  out = subprocess.run([sys.executable, '-c', code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-  assert 'BN3_OK' in out.stdout, out.stdout[-1500:]
+  calls = [('test_bn_forward_backward', (shape, relu, res)) for relu, res in ((True, False), (False, False), (True, True))]
+  for ran in run_isolated('test_bn_gpu', calls, {'RIGL_BN_FUSED': '0'}):
+    assert_ran(ran, r'k_bn_', shape)
+    assert_not_ran(ran, r'k_bn_(fwd|bwd)_fused', shape)
 
 
 @pytest.mark.parametrize('shape', [(4, 8, 8, 64), (2, 14, 14, 256), (3, 5, 9, 24)])
@@ -171,12 +170,17 @@ def test_maxpool_same_forward_backward(shape):
 # (n, h, w, cin, cout, k, stride, epilogue statistics expected): the halo kernels (3x3/s1, <= 64 channels) and the
 # space-to-depth stem have no statistics epilogue and fall back to the stats pass; the rest covers the K-major
 # kernel with both tile widths, several N tiles (cout 512 / 1024), pixel grids that do not fill their boxes (7x7, 13x9) and
-# problems with many tiles per CTA.
-@pytest.mark.parametrize('case', [(4, 56, 56, 64, 64, 3, 1, None), (4, 16, 16, 64, 128, 3, 1, True), (2, 28, 28, 128, 256, 1, 1, True),
-                                  (8, 14, 14, 64, 64, 3, 2, True), (3, 32, 32, 3, 64, 7, 2, False),
-                                  (1, 8, 8, 64, 64, 1, 1, True), (16, 7, 7, 256, 1024, 1, 1, True),
-                                  (5, 13, 9, 128, 512, 1, 1, True), (64, 56, 56, 64, 256, 1, 1, True),
-                                  (32, 28, 28, 128, 128, 3, 1, True), (6, 14, 14, 256, 256, 3, 2, True)])
+# problems with many tiles per CTA, and ragged output widths (200 = a 128-wide tile + 72 channels, 72 = a partially
+# valid second slab).
+_BN_STATS_CASES = [(4, 56, 56, 64, 64, 3, 1, None), (4, 16, 16, 64, 128, 3, 1, True), (2, 28, 28, 128, 256, 1, 1, True),
+                   (8, 14, 14, 64, 64, 3, 2, True), (3, 32, 32, 3, 64, 7, 2, False),
+                   (1, 8, 8, 64, 64, 1, 1, True), (16, 7, 7, 256, 1024, 1, 1, True),
+                   (5, 13, 9, 128, 512, 1, 1, True), (64, 56, 56, 64, 256, 1, 1, True),
+                   (32, 28, 28, 128, 128, 3, 1, True), (6, 14, 14, 256, 256, 3, 2, True),
+                   (4, 16, 16, 128, 200, 3, 1, True), (4, 14, 14, 256, 72, 1, 1, True)]
+
+
+@pytest.mark.parametrize('case', _BN_STATS_CASES)
 def test_conv_epilogue_bn_stats_match_stats_pass(case):
   """BN fed by the conv epilogue's statistics == BN with its own stats pass: both sum the bf16-ROUNDED
   outputs, in different orders (fp32 partials, fp64 combine)."""
@@ -209,6 +213,14 @@ def test_conv_epilogue_bn_stats_match_stats_pass(case):
   assert float((ma - mb).abs().max()) <= 1e-5 * float(vb.sqrt().max()) * 10 + 1e-6
   assert torch.allclose(va, vb, rtol=1e-4, atol=1e-6)
   assert float((a - b).abs().max()) <= 2 ** -7 * float(b.abs().max()) + 1e-3
+
+
+def test_conv_epilogue_bn_stats_with_cluster_multicast():
+  """The statistics epilogue in the 2-CTA multicast kernels (RIGL_CLUSTER_MC=1, read once per process)."""
+  cases = [_BN_STATS_CASES[1], _BN_STATS_CASES[-2]]
+  calls = [('test_conv_epilogue_bn_stats_match_stats_pass', (c,)) for c in cases]
+  for case, ran in zip(cases, run_isolated('test_bn_gpu', calls, {'RIGL_CLUSTER_MC': '1'})):
+    assert_ran(ran, r'k_igemm_kmajor<\d+, ?\d+, ?2>', case)
 
 
 def test_conv_epilogue_bn_stats_only_where_profitable():

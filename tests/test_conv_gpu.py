@@ -15,6 +15,9 @@ from rigl_b200 import _cabi
 from rigl_b200.layers import SparseConv2d, SparseLinear
 from rigl_b200 import pruning
 
+from isolated import assert_not_ran, assert_ran, run_isolated
+from tile_masks import STRUCTURED_CONV_CASES, STRUCTURED_LINEAR_CASES, tile_counts, tile_mask
+
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
 
@@ -59,10 +62,22 @@ CONV_CASES = [
     (2, 15, 15, 32, 64, 3, 2, 0.5, 'SAME'),
     (2, 16, 16, 32, 64, 1, 2, 0.2, 'VALID'),
     (2, 9, 9, 16, 16, 3, 1, 0.3, 'VALID'),
+    # ragged channel counts above 64: partially valid second 64-channel slab of a 128-wide N tile (fprop cout,
+    # dgrad cin), N tiles that start at channel 128 with a few channels valid, ragged K blocks; two or more M tiles
+    # in fprop and in every dgrad parity class (so the 2-CTA multicast kernels take them too)
+    (4, 8, 8, 72, 136, 1, 1, 0.5),
+    (4, 16, 16, 96, 200, 1, 2, 0.6),
+    (4, 8, 8, 200, 72, 3, 1, 0.7),
+    (4, 16, 16, 136, 200, 3, 2, 0.8),
+    (3, 7, 7, 72, 72, 3, 1, 0.5),
+    (4, 11, 11, 200, 136, 3, 2, 0.6, 'SAME'),
 ]
+RAGGED_CASES = CONV_CASES[-6:]
 
 
-def _conv_case(case, force_simt):
+def _conv_case(case, force_simt, mask=None):
+  """`mask`: None (uniformly random at the case's sparsity) or a tile_masks pattern name (dead 64x64 weight tiles;
+  the sparsity then applies inside the live tiles)."""
   n, h, w, cin, cout, k, stride, sparsity = case[:8]
   padding = case[8] if len(case) > 8 else 'FIXED'
   rng = np.random.RandomState(abs(hash(case[:8])) % (2 ** 31))
@@ -71,7 +86,10 @@ def _conv_case(case, force_simt):
   try:
     layer = SparseConv2d(cin, cout, k, strides=stride, padding=padding, name='t', device=DEV)
     w_np = _bf16(rng.standard_normal((k, k, cin, cout)) / np.sqrt(k * k * cin)).float().numpy()
-    m_np = orc.get_mask_random_numpy((k, k, cin, cout), sparsity, rng).astype(np.float32)
+    if mask is None:
+      m_np = orc.get_mask_random_numpy((k, k, cin, cout), sparsity, rng).astype(np.float32)
+    else:
+      m_np = tile_mask(mask, (k, k, cin, cout), rng, sparsity)
     with torch.no_grad():
       layer.weight.copy_(torch.from_numpy(w_np))
     layer.mask.assign(m_np)
@@ -112,40 +130,60 @@ def test_conv_default_path(case):
 
 
 LINEAR_CASES = [(1, 3, 5, 0.5), (100, 784, 300, 0.9), (100, 300, 100, 0.81), (100, 100, 10, 0.0),
-                (256, 2048, 1000, 0.85), (37, 64, 64, 0.3)]
+                (256, 2048, 1000, 0.85), (37, 64, 64, 0.3), (130, 200, 200, 0.6), (64, 136, 72, 0.5)]
+
+
+def _linear_case(case, force_simt, out='f32', use_bias=True, mask=None):
+  """`out`: 'f32' or 'bf16' output; `mask` as in _conv_case.  bf16 output without a bias takes the TMA-store
+  epilogue, fp32 output or a bias the per-thread stores."""
+  m_rows, n_in, n_out, sparsity = case
+  out_dtype = {'f32': torch.float32, 'bf16': torch.bfloat16}[out]
+  rng = np.random.RandomState(m_rows + n_in)
+  pruning.reset_default_registry()
+  _cabi.lib().rigl_set_force_simt(1 if force_simt else 0)
+  try:
+    layer = SparseLinear(n_in, n_out, use_bias=use_bias, name='fc', device=DEV, out_dtype=out_dtype)
+    w_np = _bf16(rng.standard_normal((n_in, n_out)) / np.sqrt(n_in)).float().numpy()
+    if mask is None:
+      m_np = orc.get_mask_random_numpy((n_in, n_out), sparsity, rng).astype(np.float32)
+    else:
+      m_np = tile_mask(mask, (n_in, n_out), rng, sparsity)
+    b_np = rng.standard_normal(n_out).astype(np.float32) if use_bias else None
+    with torch.no_grad():
+      layer.weight.copy_(torch.from_numpy(w_np))
+      if use_bias:
+        layer.bias.copy_(torch.from_numpy(b_np))
+    layer.mask.assign(m_np)
+    x_np = _bf16(rng.standard_normal((m_rows, n_in))).float().numpy()
+    x = torch.from_numpy(x_np).to(DEV).to(torch.bfloat16).requires_grad_(True)
+    y = layer(x)
+    assert y.dtype == out_dtype
+    y_want = orc.masked_linear_fwd(x_np, w_np, m_np, b_np)
+    (_check_f32 if out_dtype == torch.float32 else _check_bf16)(y, y_want, 'linear fprop %s' % (case,))
+    dy_np = _bf16(rng.standard_normal(y_want.shape)).float().numpy()
+    y.backward(torch.from_numpy(dy_np).to(DEV).to(out_dtype))
+    dx_want, dw_dense, dw_masked = orc.masked_linear_bwd(x_np, w_np, m_np, dy_np)
+    _check_bf16(x.grad, dx_want, 'linear dgrad %s' % (case,))
+    _check_f32(layer.masked_weights.dense_grad.view(n_in, n_out), dw_dense, 'linear dense wgrad %s' % (case,))
+    _check_f32(layer.weight.grad, dw_masked, 'linear masked wgrad %s' % (case,))
+    if use_bias:
+      _check_f32(layer.bias.grad, dy_np.astype(np.float64).sum(0), 'bias grad')
+  finally:
+    _cabi.lib().rigl_set_force_simt(0)
 
 
 @pytest.mark.parametrize('case', LINEAR_CASES)
 @pytest.mark.parametrize('force_simt', [True, False])
 def test_linear(case, force_simt):
-  m_rows, n_in, n_out, sparsity = case
-  rng = np.random.RandomState(m_rows + n_in)
-  pruning.reset_default_registry()
-  _cabi.lib().rigl_set_force_simt(1 if force_simt else 0)
-  try:
-    layer = SparseLinear(n_in, n_out, name='fc', device=DEV, out_dtype=torch.float32)
-    w_np = _bf16(rng.standard_normal((n_in, n_out)) / np.sqrt(n_in)).float().numpy()
-    m_np = orc.get_mask_random_numpy((n_in, n_out), sparsity, rng).astype(np.float32)
-    b_np = rng.standard_normal(n_out).astype(np.float32)
-    with torch.no_grad():
-      layer.weight.copy_(torch.from_numpy(w_np))
-      layer.bias.copy_(torch.from_numpy(b_np))
-    layer.mask.assign(m_np)
-    x_np = _bf16(rng.standard_normal((m_rows, n_in))).float().numpy()
-    x = torch.from_numpy(x_np).to(DEV).to(torch.bfloat16).requires_grad_(True)
-    y = layer(x)
-    assert y.dtype == torch.float32
-    y_want = orc.masked_linear_fwd(x_np, w_np, m_np, b_np)
-    _check_f32(y, y_want, 'linear fprop')
-    dy_np = _bf16(rng.standard_normal(y_want.shape)).float().numpy()
-    y.backward(torch.from_numpy(dy_np).to(DEV))
-    dx_want, dw_dense, dw_masked = orc.masked_linear_bwd(x_np, w_np, m_np, dy_np)
-    _check_bf16(x.grad, dx_want, 'linear dgrad')
-    _check_f32(layer.masked_weights.dense_grad.view(n_in, n_out), dw_dense, 'linear dense wgrad')
-    _check_f32(layer.weight.grad, dw_masked, 'linear masked wgrad')
-    _check_f32(layer.bias.grad, dy_np.astype(np.float64).sum(0), 'bias grad')
-  finally:
-    _cabi.lib().rigl_set_force_simt(0)
+  _linear_case(case, force_simt)
+
+
+@pytest.mark.parametrize('case', [c for c in LINEAR_CASES if c[2] in (1000, 200, 72)])
+@pytest.mark.parametrize('use_bias', [False, True])
+def test_linear_bf16_output(case, use_bias):
+  """The default bf16 output: without a bias through the TMA-store epilogue (ragged last N tiles of 1000, 200 and
+  72 units), with one through the per-thread bf16 stores."""
+  _linear_case(case, False, 'bf16', use_bias)
 
 
 def test_rank_and_channel_errors():
@@ -191,21 +229,29 @@ def test_conv_stem_patch_matrix_path(case):
     layers.STEM_S2D_PATH = old
 
 
+_MC = {'RIGL_CLUSTER_MC': '1'}
+_KMAJOR = r'k_igemm_kmajor<'
+_KMAJOR_MC = r'k_igemm_kmajor<\d+, ?\d+, ?2>'
+_KMAJOR_MC64 = r'k_igemm_kmajor<64, ?7, ?2>'
+
+
+def _isolated(calls, env, timeout=300):
+  """run_isolated over this module's case functions."""
+  return run_isolated('test_conv_gpu', calls, env, timeout)
+
+
 @pytest.mark.parametrize('case', [CONV_CASES[5], CONV_CASES[8], CONV_CASES[10], CONV_CASES[11]])
 def test_conv_cluster_multicast_path(case):
-  """Same results with the 2-CTA multicast clusters (run in a subprocess: the switch is read once)."""
-  import os, subprocess, sys
-  code = ('import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_conv_gpu as t; '
-          't._conv_case(%r, False); print("MC_OK")' % (os.path.dirname(os.path.dirname(__file__)),
-                                                       os.path.dirname(__file__), case))
-  env = dict(os.environ, RIGL_CLUSTER_MC='1', RIGL_CTA_PAIR='0')
-  out = subprocess.run([sys.executable, '-c', code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-  assert 'MC_OK' in out.stdout, out.stdout[-1500:]
+  """Same results with the 2-CTA multicast clusters (RIGL_CLUSTER_MC=1, read once per process)."""
+  ran, = _isolated([('_conv_case', (case, False))], _MC)
+  if case[3] % 8 == 0:                     # (the 3-channel stem runs on its own kernels)
+    assert_ran(ran, _KMAJOR_MC, case)
 
 
 # 3x3 / stride 1 / pad 1 layers with <= 64 reduction channels run on the halo kernels (one halo tile in
 # shared memory feeds all nine taps): full and partial channel blocks, H not a multiple of the strip,
-# H smaller than a strip, several N tiles, every halo pitch (16 / 32 / 64).
+# H smaller than a strip, several N tiles, every halo pitch (8 / 16 / 32 / 64 / 128).  At pitch 128 (W = 96..126) the
+# shared memory only fits one-row strips with two halo tiles in flight.
 HALO_CASES = [
     (2, 14, 14, 64, 64, 3, 1, 0.6),
     (3, 56, 56, 64, 64, 3, 1, 0.64),
@@ -213,6 +259,8 @@ HALO_CASES = [
     (2, 13, 27, 64, 24, 3, 1, 0.5),
     (5, 6, 14, 16, 64, 3, 1, 0.3),
     (2, 28, 28, 64, 64, 3, 1, 0.9, 'SAME'),
+    (2, 37, 6, 64, 64, 3, 1, 0.5),          # pitch 8
+    (1, 45, 112, 32, 64, 3, 1, 0.6),        # pitch 128
 ]
 
 
@@ -221,16 +269,20 @@ def test_conv_halo_path(case):
   _conv_case(case, force_simt=False)
 
 
+def test_conv_halo_pitches_run_the_halo_kernels():
+  """The pitch-8 and pitch-128 cases really run on the halo kernels (fprop, dgrad and wgrad)."""
+  for case, ran in zip(HALO_CASES[-2:], _isolated([('_conv_case', (c, False)) for c in HALO_CASES[-2:]], {})):
+    assert_ran(ran, r'k_halo3x3_kmajor', case)
+    assert_ran(ran, r'k_halo3x3_wgrad', case)
+    assert_not_ran(ran, _KMAJOR, case)
+
+
 @pytest.mark.parametrize('case', [HALO_CASES[1], HALO_CASES[3]])
 def test_conv_halo_disabled_matches(case):
   """RIGL_HALO3X3=0 routes the same layers through the generic per-tap kernels."""
-  import os, subprocess, sys
-  code = ('import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_conv_gpu as t; '
-          't._conv_case(%r, False); print("GEN_OK")' % (os.path.dirname(os.path.dirname(__file__)),
-                                                        os.path.dirname(__file__), case))
-  env = dict(os.environ, RIGL_HALO3X3='0')
-  out = subprocess.run([sys.executable, '-c', code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-  assert 'GEN_OK' in out.stdout, out.stdout[-1500:]
+  ran, = _isolated([('_conv_case', (case, False))], {'RIGL_HALO3X3': '0'})
+  assert_ran(ran, _KMAJOR, case)
+  assert_not_ran(ran, r'k_halo3x3', case)
 
 
 # ---- BASELINE-size problems (C2: ResNet-50, batch 256, 224x224): many more tiles than CTAs, so the persistent
@@ -348,13 +400,9 @@ def test_conv_wgrad_in_kernel_splitk_fixup_path(case):
   """RIGL_WGRAD_FIXUP=1 (opt-in; measured slower on the BASELINE shapes): the dense wgrad's split-K partials are
   summed by the last-arriving CTA inside the wgrad kernel instead of by a separate k_splitk_reduce launch.  Same
   oracle, same tolerance."""
-  import os, subprocess, sys
-  code = ('import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_conv_gpu as t; '
-          't._conv_case(%r, False); print("RED_OK")' % (os.path.dirname(os.path.dirname(__file__)),
-                                                        os.path.dirname(__file__), case))
-  env = dict(os.environ, RIGL_WGRAD_FIXUP='1')
-  out = subprocess.run([sys.executable, '-c', code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-  assert 'RED_OK' in out.stdout, out.stdout[-1500:]
+  ran, = _isolated([('_conv_case', (case, False))], {'RIGL_WGRAD_FIXUP': '1'})
+  assert_ran(ran, r'k_igemm_wgrad<', case)
+  assert_not_ran(ran, r'k_splitk_reduce', case)
 
 
 def test_conv_wgrad_accumulates_over_backward_passes():
@@ -398,3 +446,106 @@ def test_depthwise3x3_vs_fp64(case):
   _check_bf16(y.permute(0, 2, 3, 1), y64.detach().permute(0, 2, 3, 1).numpy(), 'depthwise fprop %s' % (case,))
   _check_bf16(x.grad.permute(0, 2, 3, 1), x64.grad.permute(0, 2, 3, 1).numpy(), 'depthwise dgrad %s' % (case,))
   _check_f32(dw.weight.grad, w64.grad.numpy(), 'depthwise wgrad %s' % (case,))
+
+
+# ---- dead weight tiles (tile_masks.py): the survivor-table lookups that let the K-major kernels skip the load and
+# the MMA of an all-zero 64x64 weight tile.  Run in a child process with a time limit, because a producer and
+# consumers that disagree on which K blocks are live would wait on each other forever.
+@pytest.mark.parametrize('env', [{}, _MC], ids=['default', 'cluster_mc'])
+def test_conv_dead_weight_tiles(env):
+  ran = _isolated([('_conv_case', (case, False, pattern)) for case, pattern in STRUCTURED_CONV_CASES], env, 600)
+  for (case, pattern), names in zip(STRUCTURED_CONV_CASES, ran):
+    if case[3] <= 64 and case[6] == 1:      # the halo case: its kernels keep all nine taps' weights resident
+      assert_ran(names, r'k_halo3x3_kmajor', (case, pattern))
+    else:
+      assert_ran(names, _KMAJOR_MC if env else _KMAJOR, (case, pattern))
+
+
+@pytest.mark.parametrize('env', [{}, _MC], ids=['default', 'cluster_mc'])
+def test_linear_dead_weight_tiles_at_the_liveness_cap(env):
+  """K = 320 blocks (dead blocks skipped) and 321 blocks (every block loaded) in fprop and in dgrad."""
+  calls = [('_linear_case', (case, False, 'f32', True, pattern)) for case, pattern in STRUCTURED_LINEAR_CASES]
+  for (case, pattern), names in zip(STRUCTURED_LINEAR_CASES, _isolated(calls, env, 600)):
+    assert_ran(names, _KMAJOR_MC if env else _KMAJOR, (case, pattern))
+
+
+@pytest.mark.parametrize('env', [_MC, {'RIGL_TMA_STORE': '0'}], ids=['cluster_mc', 'tma_store_0'])
+def test_conv_ragged_channels_variants(env):
+  """The ragged channel counts (in-process under the default environment: CONV_CASES) with the 2-CTA multicast and
+  with RIGL_TMA_STORE=0, the per-thread bf16 stores (fprop, and dgrad through the stride-2 parity offsets); plus a
+  bf16 linear layer without a bias (TMA store by default)."""
+  calls = [('_conv_case', (c, False)) for c in RAGGED_CASES] + \
+      [('_linear_case', ((130, 200, 200, 0.6), False, 'bf16', False))]
+  for case, names in zip(RAGGED_CASES + [None], _isolated(calls, env)):
+    assert_ran(names, _KMAJOR_MC if 'RIGL_CLUSTER_MC' in env else _KMAJOR, case)
+
+
+def test_conv_cluster_multicast_64_wide_odd_m_tiles():
+  """3 M tiles (16x8x1-pixel boxes): the partner of the last tile lies past the grid.  64-wide N tiles in
+  multicast mode: fprop of the first case, dgrad of the second."""
+  cases = [(3, 8, 16, 128, 64, 1, 1, 0.5), (3, 8, 16, 64, 256, 1, 1, 0.5)]
+  for case, ran in zip(cases, _isolated([('_conv_case', (c, False)) for c in cases], _MC)):
+    assert_ran(ran, _KMAJOR_MC64, case)
+
+
+def test_conv_cluster_multicast_with_wgrad_fixup():
+  """RIGL_CLUSTER_MC=1 and RIGL_WGRAD_FIXUP=1 together: the split-K fix-up in the multicast wgrad kernel."""
+  cases = [CONV_CASES[8], RAGGED_CASES[3]]
+  for case, ran in zip(cases, _isolated([('_conv_case', (c, False)) for c in cases], dict(_MC, RIGL_WGRAD_FIXUP='1'))):
+    assert_ran(ran, r'k_igemm_wgrad<\d+, ?\d+, ?2>', case)
+    assert_ran(ran, _KMAJOR_MC, case)
+    assert_not_ran(ran, r'k_splitk_reduce', case)
+
+
+def _packed_layout(taps, cin, cout):
+  """Mirror of packed_layout() in rigl_b200/csrc/conv_common.cuh: (off_fprop, off_dgrad, off_nnz, total, cin_pad,
+  cout_pad, n_tiles, k_tiles) of the packed operand blob."""
+  up = lambda v: (v + 255) // 256 * 256
+  cin_pad, cout_pad = (cin + 7) // 8 * 8, (cout + 7) // 8 * 8
+  n_tiles, k_tiles = (cout + 63) // 64, (cin + 63) // 64
+  off_dgrad = up(taps * cout * cin_pad * 2)
+  off_nnz = off_dgrad + up(taps * cin * cout_pad * 2)
+  return 0, off_dgrad, off_nnz, off_nnz + up(taps * n_tiles * k_tiles * 4), cin_pad, cout_pad, n_tiles, k_tiles
+
+
+def _bf16_bits(a):
+  return torch.from_numpy(np.ascontiguousarray(a, np.float32)).to(torch.bfloat16).view(torch.int16).numpy()
+
+
+_PACK_LAYERS = [((64, 256, 1), None), ((128, 128, 3), None), ((72, 200, 3), None), ((300, 100, None), None)] + \
+    [((c[3], c[4], c[5]), p) for c, p in STRUCTURED_CONV_CASES]
+
+
+@pytest.mark.parametrize('spec,pattern', _PACK_LAYERS)
+def test_pack_matches_numpy_reference(spec, pattern):
+  """rigl_pack_masked_weights against numpy: the survivor count of every 64x64 tile, both bf16 K-major operands
+  (mask * W, exactly) and zeros in the channel padding of each."""
+  cin, cout, k = spec
+  rng = np.random.RandomState(cin + cout)
+  pruning.reset_default_registry()
+  shape = (cin, cout) if k is None else (k, k, cin, cout)
+  layer = SparseLinear(cin, cout, name='fc', device=DEV) if k is None else \
+      SparseConv2d(cin, cout, k, padding='FIXED', name='c', device=DEV)
+  w_np = _bf16(rng.standard_normal(shape)).float().numpy()
+  m_np = orc.get_mask_random_numpy(shape, 0.7, rng).astype(np.float32) if pattern is None else \
+      tile_mask(pattern, shape, rng)
+  with torch.no_grad():
+    layer.weight.copy_(torch.from_numpy(w_np))
+  layer.mask.assign(m_np)
+  layer.packed.fill_(0x5a)                    # padding that is never written would show up as 0x5a5a
+  layer.pack()
+  blob = layer.packed.cpu().numpy()
+  taps = 1 if k is None else k * k
+  off_f, off_d, off_n, total, cin_pad, cout_pad, n_tiles, k_tiles = _packed_layout(taps, cin, cout)
+  assert blob.size == total
+  wm = np.where(m_np != 0, w_np, 0).reshape(taps, cin, cout)          # (no -0.0 from masked negative weights)
+  want_f = np.zeros((taps, cout, cin_pad), np.int16)
+  want_f[:, :, :cin] = _bf16_bits(wm.transpose(0, 2, 1))
+  got_f = blob[off_f:off_f + taps * cout * cin_pad * 2].view(np.int16).reshape(taps, cout, cin_pad)
+  assert np.array_equal(got_f, want_f), 'fprop operand [tap][cout][cin_pad]'
+  want_d = np.zeros((taps, cin, cout_pad), np.int16)
+  want_d[:, :, :cout] = _bf16_bits(wm)
+  got_d = blob[off_d:off_d + taps * cin * cout_pad * 2].view(np.int16).reshape(taps, cin, cout_pad)
+  assert np.array_equal(got_d, want_d), 'dgrad operand [tap][cin][cout_pad]'
+  got_n = blob[off_n:off_n + taps * n_tiles * k_tiles * 4].view(np.uint32).reshape(taps, n_tiles, k_tiles)
+  assert np.array_equal(got_n, tile_counts(m_np)), 'survivor counts [tap][cout tile][cin tile]'
