@@ -237,7 +237,7 @@ RIGL_API int rigl_masked_conv2d_fprop_bnstats(const rigl_conv_desc* d, const voi
                                               size_t ws_bytes, void* stream);
 /* The statistics epilogue is used only where it is profitable (reduction length taps*cin >= 512, or >= 256 with
  * <= 128 output channels; otherwise RIGL_ERR_UNSUPPORTED and the caller runs the plain call + a stats pass).
- * on != 0: for every supported shape (tests; same as RIGL_BN_STATS_ALWAYS=1). */
+ * on != 0: for every supported shape (tests). */
 RIGL_API int rigl_set_bn_stats_always(int on);
 /* dx = conv^T(dy, mask*W). */
 RIGL_API int rigl_masked_conv2d_dgrad(const rigl_conv_desc* d, const void* dy, const void* packed,
@@ -252,7 +252,8 @@ RIGL_API int rigl_conv2d_wgrad_dense(const rigl_conv_desc* d, const void* x, con
  * runs as a masked dense layer over [pixels, k*k*cin] with the SAME HWIO weights and mask. */
 RIGL_API int rigl_im2col_nhwc(const rigl_conv_desc* d, const void* x, void* out, int64_t out_pitch,
                               void* stream);
-/* EXPERIMENTAL (opt-in in the host mirror: layers.STEM_S2D_PATH; not yet validated on hardware).
+/* Space-to-depth stem: the host mirror's default for the ResNet stem (RIGL_STEM_S2D=0 there selects
+ * the patch matrix instead).
  * The 7x7 / stride-2 / 3-channel stem (conv2d_fixed_padding, resnet_model.py:619-629) without a
  * patch matrix: rigl_stem_s2d_fold_input folds the zero-padded input 2x2 -> 16 channels
  * ([N,(H+6)/2,(W+6)/2,16] bf16, rigl_stem_s2d_folded_bytes), the conv becomes a 4x4 stride-1 conv
@@ -271,24 +272,6 @@ RIGL_API int rigl_stem_s2d_fprop(const rigl_conv_desc* d, const void* xs, const 
                                  void* stream);
 RIGL_API int rigl_stem_s2d_wgrad(const rigl_conv_desc* d, const void* xs, const void* dy, float* dw,
                                  float beta, void* ws, size_t ws_bytes, void* stream);
-
-/* Small-Cin convs (cin <= 8, ksize <= 8: the 7x7x3 stem, resnet_model.py:620-633) WITHOUT a
- * patch matrix: the input is copied once into a zero-bordered 8-channel buffer `xp`
- * (rigl_smallc_padded_bytes); window tensor maps with a W stride of `stride` pixels then feed
- * the same tensor-core kernels with ksize "taps" of K = 64 = 8 pixels x 8 channels.  `packed` here
- * is the stem-specific operand written by rigl_smallc_pack_weights from the SAME HWIO weights
- * and mask.  dw is the dense HWIO gradient as in rigl_conv2d_wgrad_dense. */
-RIGL_API int rigl_smallc_supported(const rigl_conv_desc* d);
-RIGL_API size_t rigl_smallc_padded_bytes(const rigl_conv_desc* d);
-RIGL_API size_t rigl_smallc_packed_bytes(const rigl_conv_desc* d);
-RIGL_API size_t rigl_smallc_workspace_bytes(const rigl_conv_desc* d);
-RIGL_API int rigl_smallc_pad_input(const rigl_conv_desc* d, const void* x, void* xp, void* stream);
-RIGL_API int rigl_smallc_pack_weights(const rigl_conv_desc* d, const float* w_hwio,
-                                      const uint32_t* mask_bits, void* packed, void* stream);
-RIGL_API int rigl_smallc_fprop(const rigl_conv_desc* d, const void* xp, const void* packed, void* y,
-                               void* stream);
-RIGL_API int rigl_smallc_wgrad(const rigl_conv_desc* d, const void* xp, const void* dy, float* dw,
-                               float beta, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * Fused batch-norm (+ReLU, +residual) over NHWC bf16 activations viewed as [rows, channels]

@@ -291,13 +291,6 @@ static bool halo_geom(const ConvGeom& g, int kred, HaloParams* p, size_t smem_fi
       if (r >= g.in_h) break;
     }
   if (best_t == 0) return false;
-  if (g_halo_t > 0 && g_halo_nbuf >= 2 && g_halo_nbuf <= 4) {        // experiment override (RIGL_HALO_CFG=T,NBUF)
-    const int r = rt * g_halo_t;
-    const size_t a_buf = ((size_t)((r + 2) * wp + 8) * 128 + 1023) / 1024 * 1024;
-    if (smem_fixed + g_halo_nbuf * (a_buf + (dy_tile ? (size_t)r * wp * 128 : 0)) + 2048 <= 227 * 1024) {
-      best_t = g_halo_t; best_nbuf = g_halo_nbuf;
-    }
-  }
   p->W = g.in_w; p->H = g.in_h; p->NB = g.batch; p->Wp = wp;
   p->T = best_t; p->R = rt * best_t; p->nbuf = best_nbuf;
   p->strips_per_image = (g.in_h + p->R - 1) / p->R;

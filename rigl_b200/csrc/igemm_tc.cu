@@ -71,7 +71,6 @@ struct IgemmParams {
   int nnz_tap_stride, nnz_n_stride, nnz_k_stride;
   int tma_store;                    // 1: epilogue stages bf16 tiles in smem and TMA-stores them
   float* bn_partial;                // optional [gridDim.x][2][N]: per-CTA column sums / sums of squares of D
-  int stats_dbg;                    // development: 1 = statistics without the global REDs, 2 = without the smem pass
 };
 
 struct TMaps4 {
@@ -125,14 +124,13 @@ __device__ __forceinline__ bool build_live_mask(const IgemmParams& p, int n_tile
 // each table entry is only ever touched by one lane of one warp, in tile order, so the fp32 sums are deterministic.
 // Rows outside the pixel grid are written as zeros by their owner (see stage_slab), so they do not count.
 __device__ __forceinline__ void slab_bn_stats(uint32_t slab, int quad, int lane, float* __restrict__ bn_row, int co0,
-                                              int n, int dbg) {
+                                              int n) {
   const int cp = lane & 7, g = lane >> 3;
   const uint32_t chunk = (uint32_t)(2 * quad + (cp >> 2));
   const uint32_t word = (uint32_t)(cp & 3) * 4u;
   float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-  const int n_it = (dbg & 2) ? 0 : 32;
 #pragma unroll 8
-  for (int i = 0; i < n_it; ++i) {
+  for (int i = 0; i < 32; ++i) {
     const uint32_t row = (uint32_t)(32 * g + ((i + 2 * g) & 31));
     uint32_t v;
     asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(slab + row * 128u + (((chunk ^ (row & 7u)) << 4) | word)));
@@ -146,7 +144,7 @@ __device__ __forceinline__ void slab_bn_stats(uint32_t slab, int quad, int lane,
     q0 += __shfl_xor_sync(0xffffffffu, q0, o); q1 += __shfl_xor_sync(0xffffffffu, q1, o);
   }
   const int co = co0 + 16 * quad + 2 * cp;
-  if (g == 0 && co < n && !(dbg & 1)) {          // (n is a multiple of 8 on this path, so co + 1 < n as well)
+  if (g == 0 && co < n) {          // (n is a multiple of 8 on this path, so co + 1 < n as well)
     atomicAdd(bn_row + co, s0); atomicAdd(bn_row + co + 1, s1);
     atomicAdd(bn_row + n + co, q0); atomicAdd(bn_row + n + co + 1, q1);
   }
@@ -349,7 +347,7 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
             tma_store_4d(&omap, slab, co0, tw * p.bw, th * p.bh, tn * p.bn);
             tma_store_commit();
           }
-          if (bn_row && wg == 0) slab_bn_stats(slab, cw, lane, bn_row, co0, p.N, p.stats_dbg);   // next to the bulk store's own read
+          if (bn_row && wg == 0) slab_bn_stats(slab, cw, lane, bn_row, co0, p.N);   // next to the bulk store's own read
           ++slab_ctr;
         }
       } else {
@@ -391,9 +389,6 @@ struct WgradParams {
   int m_tiles, n_tiles;
   float* out;                       // [splits][taps][ci][co] partials (or dw itself when splits == 1)
   long long split_stride;           // elements between split slices
-  int* counters;                    // split-K fix-up: arrivals per output tile (zeroed by the launcher), or null
-  float* dw;                        // fix-up target [taps][ci][co]
-  float beta;                       // dw <- beta * dw + sum of the partials
 };
 
 // Same warp roles as k_igemm_kmajor; consumer warpgroup w owns input channels 64w..64w+63 of the unit (the
@@ -418,7 +413,6 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
 
-  __shared__ int s_last;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < 4; ++i) prefetch_tmap(&xmaps.a[i]);
@@ -532,42 +526,6 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
                 make_float2(acc[4 * jc + 2 * h], acc[4 * jc + 2 * h + 1]);
         }
       }
-      if (p.counters != nullptr) {
-        // ---- split-K fix-up inside the kernel: the unit that arrives LAST at an output tile sums the partial
-        // tiles of all splits in split order (deterministic) while they are still in L2, and writes dw.  Replaces
-        // one k_splitk_reduce launch per layer.
-        __threadfence();                                   // my part of this unit's partial tile is visible
-        named_bar_sync(2, kConsumerThreads);
-        if (cw == 0 && lane == 0) {
-          int last = 0;
-          if (live) {
-            int* ctr = p.counters + (mi * p.n_tiles + n_tile);
-            last = (atomicAdd(ctr, 1) == p.splits - 1) ? 1 : 0;
-            if (last) *ctr = 0;                            // every split has arrived: re-arm for the next launch
-          }
-          s_last = last;
-        }
-        named_bar_sync(2, kConsumerThreads);
-        if (s_last) {
-          __threadfence();
-          const long long tap_off = (long long)p.taps[tap_idx].b_tap * p.ci;
-          for (int rr = cw; rr < kBM && m0 + rr < p.ci; rr += kConsumerWarps) {   // warp per row, lanes over columns
-            const long long row_off = (tap_off + m0 + rr) * p.co;
-            for (int c = 4 * lane; c < BN; c += 128) {
-              const int co = n_tile * BN + c;
-              if (co >= p.co) break;
-              float4 a = p.beta != 0.f ? *reinterpret_cast<const float4*>(p.dw + row_off + co)
-                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-              for (int sp = 0; sp < p.splits; ++sp) {
-                const float4 v = __ldcg(reinterpret_cast<const float4*>(p.out + (long long)sp * p.split_stride + row_off + co));
-                a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
-              }
-              *reinterpret_cast<float4*>(p.dw + row_off + co) = a;
-            }
-          }
-        }
-        named_bar_sync(2, kConsumerThreads);               // s_last is rewritten by the next unit
-      }
     }
   }
   if (CL > 1) cluster_sync_all();                         // no CTA exits while its peer may still signal it
@@ -603,16 +561,11 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 static EncodeTiledFn g_encode = nullptr;
 static bool g_tma_store = true;     // RIGL_TMA_STORE=0 falls back to per-thread global stores
-// RIGL_WGRAD_FIXUP=1: the last-arriving CTA of an output tile sums the split-K partials inside the wgrad kernel
-// instead of a separate k_splitk_reduce launch.  Off by default: the layers with few output tiles run 100-300
-// splits, and one CTA then sums tens of MB that the separate kernel spreads over the whole grid.
-static bool g_wgrad_fixup = false;
 // RIGL_CLUSTER_MC=1: 2-CTA clusters whose CTAs share the weight tile (fprop/dgrad) or the dY tile (wgrad): each loads
 // half of it and multicasts it to both, halving those L2 -> SM bytes.  Opt-in; the single-CTA kernels are the default.
 static bool g_cluster_mc = false;
-static bool g_bn_stats_always = false;   // RIGL_BN_STATS_ALWAYS=1: epilogue statistics for every supported shape (tests)
+static bool g_bn_stats_always = false;   // rigl_set_bn_stats_always: epilogue statistics for every supported shape (tests)
 static bool g_halo = true;          // RIGL_HALO3X3=0: 3x3/s1 layers with <= 64 channels use the generic kernels
-static int g_halo_t = 0, g_halo_nbuf = 0;   // RIGL_HALO_CFG=T,NBUF: tuning override for the halo kernels
 static int g_num_sms = 0;
 static std::once_flag g_once;
 static int g_init_status = RIGL_OK;
@@ -629,10 +582,7 @@ static void init_driver() {
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   if (const char* e = getenv("RIGL_TMA_STORE")) g_tma_store = !(e[0] == '0');
   if (const char* e = getenv("RIGL_HALO3X3")) g_halo = !(e[0] == '0');
-  if (const char* e = getenv("RIGL_BN_STATS_ALWAYS")) g_bn_stats_always = (e[0] == '1');
-  if (const char* e = getenv("RIGL_WGRAD_FIXUP")) g_wgrad_fixup = (e[0] == '1');
   if (const char* e = getenv("RIGL_CLUSTER_MC")) g_cluster_mc = (e[0] == '1');
-  if (const char* e = getenv("RIGL_HALO_CFG")) sscanf(e, "%d,%d", &g_halo_t, &g_halo_nbuf);
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
@@ -702,6 +652,37 @@ static void choose_box(int gw, int gh, int nb, int total, int* bw, int* bh, int*
 static inline int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 static inline int posmod(int a, int b) { return ((a % b) + b) % b; }
 
+// Tiling of a launch's gw x gh x nb pixel grid by boxes of `box_pixels` pixels (IgemmParams or WgradParams).
+template <typename P>
+static void set_pixel_tiling(P& p, int gw, int gh, int nb, int box_pixels) {
+  p.GW = gw; p.GH = gh; p.NB = nb;
+  choose_box(gw, gh, nb, box_pixels, &p.bw, &p.bh, &p.bn);
+  p.tiles_w = (gw + p.bw - 1) / p.bw; p.tiles_h = (gh + p.bh - 1) / p.bh; p.tiles_n = (nb + p.bn - 1) / p.bn;
+}
+
+// Every filter tap of g reads x at its output pixels shifted by the tap offset.  With stride s, x is viewed through
+// one parity sub-grid map per (kh - pad, kw - pad) mod s (up to four); maps no tap uses alias a used one.
+template <typename P>
+static int set_conv_taps(P& p, TMaps4* maps, const ConvGeom& g, const void* x, const uint32_t box[4]) {
+  bool made[4] = {false, false, false, false};
+  p.ntaps = 0;
+  for (int kh = 0; kh < g.ksize; ++kh)
+    for (int kw = 0; kw < g.ksize; ++kw) {
+      const int rh = posmod(kh - g.pad, g.stride), rw = posmod(kw - g.pad, g.stride);
+      const int id = rh * g.stride + rw;
+      if (!made[id]) {
+        const int rc = make_act_map(&maps->a[id], x, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, g.stride, rh, rw, box);
+        if (rc != RIGL_OK) return rc;
+        made[id] = true;
+      }
+      TapInfo& t = p.taps[p.ntaps++];
+      t.map_id = (int8_t)id; t.dh = (int8_t)floordiv(kh - g.pad, g.stride); t.dw = (int8_t)floordiv(kw - g.pad, g.stride);
+      t.b_tap = kh * g.ksize + kw;
+    }
+  for (int i = 0; i < 4; ++i) if (!made[i]) maps->a[i] = maps->a[p.taps[0].map_id];
+  return RIGL_OK;
+}
+
 int tc_max_ctas() {
   ensure_driver();
   return g_num_sms > 0 ? g_num_sms : kNumSmsHint;
@@ -731,11 +712,6 @@ static size_t wgrad_ws_elems(const ConvGeom& g, int* splits_out, int* bps_out, i
   return (size_t)splits * g.taps() * g.cin * g.cout;
 }
 
-static size_t wgrad_counter_bytes(const ConvGeom& g, int bn_tile) {
-  const size_t tiles = (size_t)g.taps() * ((g.cin + kBM - 1) / kBM + 1) * ((g.cout + bn_tile - 1) / bn_tile);
-  return (tiles * sizeof(int) + 255) / 256 * 256;
-}
-
 // Wider N tiles halve the L2->smem bytes per FLOP (the wgrad main loop is L2-bandwidth bound: K blocks are
 // only 64 pixels deep); 128 is the widest whose accumulators fit the consumer warpgroups' registers.
 static int wgrad_bn_tile(const ConvGeom& g) { return g.cout >= 128 ? 128 : 64; }
@@ -750,7 +726,7 @@ size_t tc_workspace_bytes(const ConvGeom& g) {
   size_t elems = wgrad_ws_elems(g, nullptr, nullptr, bw, bh, bn, wgrad_bn_tile(g));
   HaloParams hp;
   if (halo_wgrad_ok(g, &hp)) { const size_t e = halo_wgrad_ws_elems(g, hp); if (e > elems) elems = e; }
-  return elems * sizeof(float) + wgrad_counter_bytes(g, wgrad_bn_tile(g)) + 256;
+  return elems * sizeof(float) + 256;
 }
 
 static bool kmajor_use_mc(const IgemmParams& p) {      // multicast needs a partner M tile
@@ -814,16 +790,13 @@ static int dispatch_kmajor(int n_out, const TMaps4& amaps, const CUtensorMap& bm
   return mc ? launch_kmajor<128, 5, 2>(amaps, bmap, omap, p, s) : launch_kmajor<128, 5, 1>(amaps, bmap, omap, p, s);
 }
 
-static int pick_bn(int n_out, long long m_tiles) {
+static int pick_bn(int n_out) {
   // The widest tile whose accumulators fit the consumer warpgroups' registers (64 x 128 fp32 per warpgroup):
   // fewest A re-reads.
-  (void)m_tiles;
   return n_out > 64 ? 128 : 64;
 }
 
 void tc_set_bn_stats_always(bool on) { g_bn_stats_always = on; }
-static int g_stats_dbg = 0;
-void tc_set_bn_stats_debug(int v) { g_stats_dbg = v; }
 
 int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32, const float* bias,
              void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial, int* bn_rows) {
@@ -854,9 +827,7 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
     }
   }
   IgemmParams p = {};
-  choose_box(g.out_w, g.out_h, g.batch, 128, &p.bw, &p.bh, &p.bn);
-  p.GW = g.out_w; p.GH = g.out_h; p.NB = g.batch;
-  p.tiles_w = (p.GW + p.bw - 1) / p.bw; p.tiles_h = (p.GH + p.bh - 1) / p.bh; p.tiles_n = (p.NB + p.bn - 1) / p.bn;
+  set_pixel_tiling(p, g.out_w, g.out_h, g.batch, 128);
   p.kblks = (g.cin + kBK - 1) / kBK;
   p.N = g.cout;
   p.out_bf16 = static_cast<__nv_bfloat16*>(y); p.out_f32 = y_f32; p.bias = bias;
@@ -864,26 +835,11 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
   p.nnz = reinterpret_cast<const uint32_t*>(pk + L.off_nnz);
   p.nnz_tap_stride = L.n_tiles * L.k_tiles; p.nnz_n_stride = L.k_tiles; p.nnz_k_stride = 1;
   p.bn_partial = bn_partial;            // (decides the kernel variant, hence the B box: set before the maps)
-  p.stats_dbg = g_stats_dbg;
   TMaps4 amaps;
   const uint32_t abox[4] = {(uint32_t)kBK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-  bool made[4] = {false, false, false, false};
-  p.ntaps = 0;
-  for (int kh = 0; kh < g.ksize; ++kh)
-    for (int kw = 0; kw < g.ksize; ++kw) {
-      const int rh = posmod(kh - g.pad, g.stride), rw = posmod(kw - g.pad, g.stride);
-      const int id = rh * g.stride + rw;
-      if (!made[id]) {
-        rc = make_act_map(&amaps.a[id], x, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, g.stride, rh, rw, abox);
-        if (rc != RIGL_OK) return rc;
-        made[id] = true;
-      }
-      TapInfo& t = p.taps[p.ntaps++];
-      t.map_id = (int8_t)id; t.dh = (int8_t)floordiv(kh - g.pad, g.stride); t.dw = (int8_t)floordiv(kw - g.pad, g.stride);
-      t.b_tap = kh * g.ksize + kw;
-    }
-  for (int i = 0; i < 4; ++i) if (!made[i]) amaps.a[i] = amaps.a[p.taps[0].map_id];
-  const int bn_tile = pick_bn(g.cout, (long long)p.tiles_w * p.tiles_h * p.tiles_n);
+  rc = set_conv_taps(p, &amaps, g, x, abox);
+  if (rc != RIGL_OK) return rc;
+  const int bn_tile = pick_bn(g.cout);
   CUtensorMap bmap;
   const uint64_t bdims[3] = {(uint64_t)L.cin_pad, (uint64_t)g.cout, (uint64_t)g.taps()};
   const uint64_t bstr[2] = {(uint64_t)L.cin_pad * 2, (uint64_t)g.cout * L.cin_pad * 2};
@@ -935,8 +891,8 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
   for (int ph = 0; ph < st; ++ph)
     for (int pw = 0; pw < st; ++pw) {
       IgemmParams p = {};
-      p.GH = (g.in_h - ph + st - 1) / st; p.GW = (g.in_w - pw + st - 1) / st; p.NB = g.batch;
-      if (p.GH <= 0 || p.GW <= 0) continue;
+      const int gh = (g.in_h - ph + st - 1) / st, gw = (g.in_w - pw + st - 1) / st;
+      if (gh <= 0 || gw <= 0) continue;
       p.ntaps = 0;
       for (int kh = 0; kh < g.ksize; ++kh)
         for (int kw = 0; kw < g.ksize; ++kw)
@@ -946,8 +902,7 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
             t.b_tap = kh * g.ksize + kw;
           }
       if (p.ntaps == 0) continue;
-      choose_box(p.GW, p.GH, p.NB, 128, &p.bw, &p.bh, &p.bn);
-      p.tiles_w = (p.GW + p.bw - 1) / p.bw; p.tiles_h = (p.GH + p.bh - 1) / p.bh; p.tiles_n = (p.NB + p.bn - 1) / p.bn;
+      set_pixel_tiling(p, gw, gh, g.batch, 128);
       p.kblks = (g.cout + kBK - 1) / kBK;
       p.N = g.cin;
       p.out_bf16 = static_cast<__nv_bfloat16*>(dx);
@@ -962,7 +917,7 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
       rc = make_act_map(&amaps.a[0], dy, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
       if (rc != RIGL_OK) return rc;
       for (int i = 1; i < 4; ++i) amaps.a[i] = amaps.a[0];
-      const int bn_tile = pick_bn(g.cin, (long long)p.tiles_w * p.tiles_h * p.tiles_n);
+      const int bn_tile = pick_bn(g.cin);
       CUtensorMap bmap;
       const uint64_t bdims[3] = {(uint64_t)L.cout_pad, (uint64_t)g.cin, (uint64_t)g.taps()};
       const uint64_t bstr[2] = {(uint64_t)L.cout_pad * 2, (uint64_t)g.cin * L.cout_pad * 2};
@@ -1030,9 +985,7 @@ int tc_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float 
     }
   }
   WgradParams p = {};
-  choose_box(g.out_w, g.out_h, g.batch, 64, &p.bw, &p.bh, &p.bn);
-  p.GW = g.out_w; p.GH = g.out_h; p.NB = g.batch;
-  p.tiles_w = (p.GW + p.bw - 1) / p.bw; p.tiles_h = (p.GH + p.bh - 1) / p.bh; p.tiles_n = (p.NB + p.bn - 1) / p.bn;
+  set_pixel_tiling(p, g.out_w, g.out_h, g.batch, 64);
   p.pblocks = p.tiles_w * p.tiles_h * p.tiles_n;
   const int bn_tile = wgrad_bn_tile(g);
   const size_t elems = wgrad_ws_elems(g, &p.splits, &p.pblocks_per_split, p.bw, p.bh, p.bn, bn_tile);
@@ -1042,255 +995,29 @@ int tc_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float 
   const bool direct = (p.splits == 1 && beta == 0.f);
   if (!direct) {
     const size_t need = elems * sizeof(float);
-    const size_t ctr_bytes = wgrad_counter_bytes(g, bn_tile);
-    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
-    if (ws == nullptr || ws_bytes < need + ctr_bytes + 256) {
-      set_error("rigl_conv2d_wgrad_dense: workspace %zu < required %zu", ws_bytes, need + ctr_bytes + 256);
+    if (ws == nullptr || ws_bytes < need + 256) {
+      set_error("rigl_conv2d_wgrad_dense: workspace %zu < required %zu", ws_bytes, need + 256);
       return RIGL_ERR_WORKSPACE;
     }
-    p.out = reinterpret_cast<float*>(base + ctr_bytes); p.split_stride = n_w;
-    if (g_wgrad_fixup) {
-      p.counters = reinterpret_cast<int*>(base); p.dw = dw; p.beta = beta;
-      RIGL_CUDA(cudaMemsetAsync(p.counters, 0, ctr_bytes, s));     // (the kernel re-arms them, but the scratch is the caller's)
-    }
+    p.out = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
+    p.split_stride = n_w;
   } else {
     p.out = dw; p.split_stride = 0;
   }
   TMaps4 xmaps;
   const uint32_t box[4] = {64, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-  bool made[4] = {false, false, false, false};
-  p.ntaps = 0;
-  for (int kh = 0; kh < g.ksize; ++kh)
-    for (int kw = 0; kw < g.ksize; ++kw) {
-      const int rh = posmod(kh - g.pad, g.stride), rw = posmod(kw - g.pad, g.stride);
-      const int id = rh * g.stride + rw;
-      if (!made[id]) {
-        rc = make_act_map(&xmaps.a[id], x, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, g.stride, rh, rw, box);
-        if (rc != RIGL_OK) return rc;
-        made[id] = true;
-      }
-      TapInfo& t = p.taps[p.ntaps++];
-      t.map_id = (int8_t)id; t.dh = (int8_t)floordiv(kh - g.pad, g.stride); t.dw = (int8_t)floordiv(kw - g.pad, g.stride);
-      t.b_tap = kh * g.ksize + kw;
-    }
-  for (int i = 0; i < 4; ++i) if (!made[i]) xmaps.a[i] = xmaps.a[p.taps[0].map_id];
+  rc = set_conv_taps(p, &xmaps, g, x, box);
+  if (rc != RIGL_OK) return rc;
   CUtensorMap dymap;
   rc = make_act_map(&dymap, dy, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, box);
   if (rc != RIGL_OK) return rc;
   rc = (bn_tile == 128) ? launch_wgrad<128, 6>(xmaps, dymap, p, s) : launch_wgrad<64, 8>(xmaps, dymap, p, s);
   if (rc != RIGL_OK) return rc;
-  if (!direct && p.counters == nullptr) {
+  if (!direct) {
     const long long threads = (n_w + 3) / 4;
     k_splitk_reduce<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(p.out, p.split_stride, p.splits, dw, n_w, beta);
     RIGL_LAUNCH_CHECK("k_splitk_reduce");
   }
-  return RIGL_OK;
-}
-
-// ----------------------------------------------------------------------------
-// Small-Cin convs (the 7x7x3 stem) without a patch matrix.
-// The input is copied once into a zero-bordered, 8-channel-padded buffer xp[N,Hp,Wp,8]; for
-// filter row kh the K slice (kw, c) of an output pixel is then 64 CONTIGUOUS bf16 (8 pixels x
-// 8 channels) starting at pixel (s*wo, s*ho + kh): a tensor map whose W dimension has a
-// stride of s pixels (32 bytes for s = 2: overlapping windows) presents exactly that to TMA,
-// so the conv runs on the same k_igemm_kmajor / k_igemm_wgrad kernels with k "taps" of K = 64
-// and weights packed as [kh][co][kw*8 + c].  No im2col buffer, 216 MB instead of 1 GB of traffic.
-// ----------------------------------------------------------------------------
-struct SmallCGeom {
-  int hp, wp;        // padded input extents
-};
-
-static SmallCGeom smallc_geom(const ConvGeom& g) {
-  SmallCGeom q;
-  q.hp = (g.out_h - 1) * g.stride + g.ksize;
-  q.wp = (g.out_w - 1) * g.stride + 8;
-  return q;
-}
-
-__global__ void k_smallc_pad(ConvGeom g, int hp, int wp, const __nv_bfloat16* __restrict__ x,
-                             __nv_bfloat16* __restrict__ xp) {
-  const long long total = (long long)g.batch * hp * wp;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
-       i += (long long)gridDim.x * blockDim.x) {
-    const int w = (int)(i % wp), h = (int)((i / wp) % hp), n = (int)(i / ((long long)wp * hp));
-    const int hi = h - g.pad, wi = w - g.pad;
-    __align__(16) __nv_bfloat16 v[8];
-#pragma unroll
-    for (int c = 0; c < 8; ++c) v[c] = __float2bfloat16(0.f);
-    if (hi >= 0 && hi < g.in_h && wi >= 0 && wi < g.in_w) {
-      const __nv_bfloat16* src = x + (((long long)n * g.in_h + hi) * g.in_w + wi) * g.x_pitch;
-      for (int c = 0; c < g.cin; ++c) v[c] = src[c];
-    }
-    reinterpret_cast<uint4*>(xp)[i] = *reinterpret_cast<const uint4*>(v);
-  }
-}
-
-// packed[kh][co][kw*8 + c] = mask ? w[kh,kw,c,co] : 0   (zero for c >= cin, kw >= k)
-__global__ void k_smallc_pack(ConvGeom g, const float* __restrict__ w, const uint32_t* __restrict__ bits,
-                              __nv_bfloat16* __restrict__ out) {
-  const int total = g.ksize * g.cout * 64;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int kk = i % 64, co = (i / 64) % g.cout, kh = i / (64 * g.cout);
-  const int kw = kk >> 3, c = kk & 7;
-  float v = 0.f;
-  if (kw < g.ksize && c < g.cin) {
-    const long long e = (((long long)kh * g.ksize + kw) * g.cin + c) * g.cout + co;
-    if ((bits[e >> 5] >> (e & 31)) & 1u) v = w[e];
-  }
-  out[i] = __float2bfloat16(v);
-}
-
-// dw_hwio[kh,kw,c,co] = beta*dw + sum_s part[s][kh][kw*8+c][co]
-__global__ void k_smallc_unpack(ConvGeom g, const float* __restrict__ part, long long split_stride, int splits,
-                                float* __restrict__ dw, float beta) {
-  const long long total = (long long)g.ksize * g.ksize * g.cin * g.cout;
-  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= total) return;
-  const int co = (int)(e % g.cout), c = (int)((e / g.cout) % g.cin);
-  const int kw = (int)((e / ((long long)g.cout * g.cin)) % g.ksize), kh = (int)(e / ((long long)g.cout * g.cin * g.ksize));
-  const long long src = ((long long)kh * 64 + kw * 8 + c) * g.cout + co;
-  float a = beta != 0.f ? dw[e] : 0.f;
-  for (int s = 0; s < splits; ++s) a += part[(long long)s * split_stride + src];
-  dw[e] = a;
-}
-
-bool smallc_supported(const ConvGeom& g) {
-  return g.cin <= 8 && g.ksize <= 8 && g.ksize >= 2 && g.cout % 8 == 0 && (g.stride == 1 || g.stride == 2);
-}
-
-size_t smallc_padded_bytes(const ConvGeom& g) {
-  const SmallCGeom q = smallc_geom(g);
-  return (size_t)g.batch * q.hp * q.wp * 16;
-}
-
-size_t smallc_packed_bytes(const ConvGeom& g) { return (size_t)g.ksize * g.cout * 64 * 2; }
-
-int smallc_pad_input(const ConvGeom& g, const void* x, void* xp, cudaStream_t s) {
-  const SmallCGeom q = smallc_geom(g);
-  k_smallc_pad<<<kNumSmsHint * 16, 256, 0, s>>>(g, q.hp, q.wp, (const __nv_bfloat16*)x, (__nv_bfloat16*)xp);
-  RIGL_LAUNCH_CHECK("k_smallc_pad");
-  return RIGL_OK;
-}
-
-int smallc_pack(const ConvGeom& g, const float* w, const uint32_t* bits, void* packed, cudaStream_t s) {
-  const int total = g.ksize * g.cout * 64;
-  k_smallc_pack<<<(total + 255) / 256, 256, 0, s>>>(g, w, bits, (__nv_bfloat16*)packed);
-  RIGL_LAUNCH_CHECK("k_smallc_pack");
-  return RIGL_OK;
-}
-
-// Window view of xp for filter rows kh == parity (mod stride): dims (64, out_w, rows, N).
-static int make_window_map(CUtensorMap* out, const void* xp, const ConvGeom& g, const SmallCGeom& q, int parity,
-                           const uint32_t box[4]) {
-  const uint64_t rows = (q.hp - parity + g.stride - 1) / g.stride;
-  const uint64_t dims[4] = {64, (uint64_t)g.out_w, rows, (uint64_t)g.batch};
-  const uint64_t strides[3] = {(uint64_t)g.stride * 16, (uint64_t)g.stride * q.wp * 16, (uint64_t)q.hp * q.wp * 16};
-  const uint8_t* base = static_cast<const uint8_t*>(xp) + (size_t)parity * q.wp * 16;
-  return make_tmap(out, base, 4, dims, strides, box);
-}
-
-int smallc_fprop(const ConvGeom& g, const void* xp, const void* packed, void* y, cudaStream_t s) {
-  int rc = ensure_driver();
-  if (rc != RIGL_OK) return rc;
-  const SmallCGeom q = smallc_geom(g);
-  IgemmParams p = {};
-  choose_box(g.out_w, g.out_h, g.batch, 128, &p.bw, &p.bh, &p.bn);
-  p.GW = g.out_w; p.GH = g.out_h; p.NB = g.batch;
-  p.tiles_w = (p.GW + p.bw - 1) / p.bw; p.tiles_h = (p.GH + p.bh - 1) / p.bh; p.tiles_n = (p.NB + p.bn - 1) / p.bn;
-  p.kblks = 1;
-  p.N = g.cout;
-  p.out_bf16 = static_cast<__nv_bfloat16*>(y);
-  p.o_off = 0; p.o_sw = g.cout; p.o_sh = (long long)g.out_w * g.cout; p.o_sn = (long long)g.out_h * g.out_w * g.cout;
-  p.nnz = nullptr;
-  TMaps4 amaps;
-  const uint32_t abox[4] = {64, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-  for (int par = 0; par < g.stride; ++par) {
-    rc = make_window_map(&amaps.a[par], xp, g, q, par, abox);
-    if (rc != RIGL_OK) return rc;
-  }
-  for (int i = g.stride; i < 4; ++i) amaps.a[i] = amaps.a[0];
-  p.ntaps = g.ksize;
-  for (int kh = 0; kh < g.ksize; ++kh) {
-    TapInfo& t = p.taps[kh];
-    t.map_id = (int8_t)(kh % g.stride); t.dh = (int8_t)(kh / g.stride); t.dw = 0; t.b_tap = kh;
-  }
-  const int bn_tile = pick_bn(g.cout, (long long)p.tiles_w * p.tiles_h * p.tiles_n);
-  CUtensorMap bmap;
-  const uint64_t bdims[3] = {64, (uint64_t)g.cout, (uint64_t)g.ksize};
-  const uint64_t bstr[2] = {128, (uint64_t)g.cout * 128};
-  const uint32_t bbox[3] = {64, (uint32_t)kmajor_b_rows(p, bn_tile), 1};
-  rc = make_tmap(&bmap, packed, 3, bdims, bstr, bbox);
-  if (rc != RIGL_OK) return rc;
-  CUtensorMap omap = bmap;
-  p.tma_store = g_tma_store ? 1 : 0;
-  if (p.tma_store) {
-    rc = make_act_map(&omap, y, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
-    if (rc != RIGL_OK) return rc;
-  }
-  return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s);
-}
-
-static ConvGeom smallc_as_gemm(const ConvGeom& g) {     // the wgrad work decomposition sees k taps of 64 "channels"
-  ConvGeom v = g;
-  v.ksize = 1; v.cin = 64;
-  return v;
-}
-
-size_t smallc_wgrad_ws_bytes(const ConvGeom& g) {
-  int bw, bh, bn;
-  choose_box(g.out_w, g.out_h, g.batch, 64, &bw, &bh, &bn);
-  ConvGeom v = smallc_as_gemm(g);
-  return wgrad_ws_elems(v, nullptr, nullptr, bw, bh, bn, wgrad_bn_tile(g)) * g.ksize * sizeof(float) + 256;
-}
-
-int smallc_wgrad(const ConvGeom& g, const void* xp, const void* dy, float* dw, float beta, void* ws, size_t ws_bytes,
-                 cudaStream_t s) {
-  int rc = ensure_driver();
-  if (rc != RIGL_OK) return rc;
-  const SmallCGeom q = smallc_geom(g);
-  WgradParams p = {};
-  choose_box(g.out_w, g.out_h, g.batch, 64, &p.bw, &p.bh, &p.bn);
-  p.GW = g.out_w; p.GH = g.out_h; p.NB = g.batch;
-  p.tiles_w = (p.GW + p.bw - 1) / p.bw; p.tiles_h = (p.GH + p.bh - 1) / p.bh; p.tiles_n = (p.NB + p.bn - 1) / p.bn;
-  p.pblocks = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int bn_tile = wgrad_bn_tile(g);
-  const int out_tiles = g.ksize * ((g.cout + bn_tile - 1) / bn_tile);
-  int splits = (2 * g_num_sms + out_tiles - 1) / out_tiles;
-  if (splits > p.pblocks) splits = p.pblocks;
-  if (splits < 1) splits = 1;
-  p.pblocks_per_split = (p.pblocks + splits - 1) / splits;
-  p.splits = (p.pblocks + p.pblocks_per_split - 1) / p.pblocks_per_split;
-  p.ci = 64; p.co = g.cout;
-  p.m_tiles = 1; p.n_tiles = (g.cout + bn_tile - 1) / bn_tile;
-  const long long n_part = (long long)g.ksize * 64 * g.cout;
-  const size_t need = (size_t)p.splits * n_part * sizeof(float);
-  if (ws == nullptr || ws_bytes < need + 256) {
-    set_error("rigl_smallc_wgrad: workspace %zu < required %zu", ws_bytes, need + 256);
-    return RIGL_ERR_WORKSPACE;
-  }
-  p.out = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
-  p.split_stride = n_part;
-  TMaps4 xmaps;
-  const uint32_t box[4] = {64, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-  for (int par = 0; par < g.stride; ++par) {
-    rc = make_window_map(&xmaps.a[par], xp, g, q, par, box);
-    if (rc != RIGL_OK) return rc;
-  }
-  for (int i = g.stride; i < 4; ++i) xmaps.a[i] = xmaps.a[0];
-  p.ntaps = g.ksize;
-  for (int kh = 0; kh < g.ksize; ++kh) {
-    TapInfo& t = p.taps[kh];
-    t.map_id = (int8_t)(kh % g.stride); t.dh = (int8_t)(kh / g.stride); t.dw = 0; t.b_tap = kh;
-  }
-  CUtensorMap dymap;
-  rc = make_act_map(&dymap, dy, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, box);
-  if (rc != RIGL_OK) return rc;
-  rc = (bn_tile == 128) ? launch_wgrad<128, 6>(xmaps, dymap, p, s) : launch_wgrad<64, 8>(xmaps, dymap, p, s);
-  if (rc != RIGL_OK) return rc;
-  const long long total = (long long)g.ksize * g.ksize * g.cin * g.cout;
-  k_smallc_unpack<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(g, p.out, p.split_stride, p.splits, dw, beta);
-  RIGL_LAUNCH_CHECK("k_smallc_unpack");
   return RIGL_OK;
 }
 

@@ -48,7 +48,7 @@ CONV_CASES = [
     (2, 9, 7, 8, 16, 3, 2, 0.8),
     (3, 8, 8, 64, 64, 1, 1, 0.0),
     (2, 14, 14, 64, 128, 1, 2, 0.4),
-    (2, 12, 12, 3, 8, 7, 2, 0.14),      # stem-like: cin=3 (small-Cin window-map path / SIMT)
+    (2, 12, 12, 3, 8, 7, 2, 0.14),      # stem-like: cin=3 (space-to-depth stem / SIMT)
     (3, 32, 32, 3, 64, 7, 2, 0.14),
     (2, 17, 17, 3, 16, 3, 1, 0.3),
     (4, 16, 16, 64, 64, 3, 1, 0.64),
@@ -195,17 +195,6 @@ def test_rank_and_channel_errors():
     layer(torch.zeros(2, 4, 4, 4, device=DEV))
 
 
-@pytest.mark.parametrize('case', [(2, 12, 12, 3, 8, 7, 2, 0.14), (3, 32, 32, 3, 64, 7, 2, 0.14), (2, 17, 17, 3, 16, 3, 1, 0.3)])
-def test_conv_stem_window_path(case):
-  """The opt-in small-Cin path (zero-bordered 8-channel input + overlapping-window tensor maps)."""
-  from rigl_b200 import layers
-  layers.STEM_WINDOW_PATH = True
-  try:
-    _conv_case(case, force_simt=False)
-  finally:
-    layers.STEM_WINDOW_PATH = False
-
-
 @pytest.mark.parametrize('case', [(2, 16, 16, 3, 64, 7, 2, 0.14), (3, 32, 32, 3, 64, 7, 2, 0.14),
                                   (2, 64, 48, 3, 16, 7, 2, 0.5), (2, 224, 224, 3, 64, 7, 2, 0.14)])
 def test_conv_stem_s2d_path(case):
@@ -233,6 +222,7 @@ _MC = {'RIGL_CLUSTER_MC': '1'}
 _KMAJOR = r'k_igemm_kmajor<'
 _KMAJOR_MC = r'k_igemm_kmajor<\d+, ?\d+, ?2>'
 _KMAJOR_MC64 = r'k_igemm_kmajor<64, ?7, ?2>'
+_WGRAD_MC = r'k_igemm_wgrad<\d+, ?\d+, ?2>'
 
 
 def _isolated(calls, env, timeout=300):
@@ -246,6 +236,8 @@ def test_conv_cluster_multicast_path(case):
   ran, = _isolated([('_conv_case', (case, False))], _MC)
   if case[3] % 8 == 0:                     # (the 3-channel stem runs on its own kernels)
     assert_ran(ran, _KMAJOR_MC, case)
+  if case[4] >= 128:                       # 128-wide wgrad N tiles: the dY tile is multicast
+    assert_ran(ran, _WGRAD_MC, case)
 
 
 # 3x3 / stride 1 / pad 1 layers with <= 64 reduction channels run on the halo kernels (one halo tile in
@@ -395,19 +387,9 @@ def test_batched_pack_equals_per_layer_pack():
   layers._PACKED_AHEAD.clear()
 
 
-@pytest.mark.parametrize('case', [CONV_CASES[8], CONV_CASES[9], CONV_CASES[11]])
-def test_conv_wgrad_in_kernel_splitk_fixup_path(case):
-  """RIGL_WGRAD_FIXUP=1 (opt-in; measured slower on the BASELINE shapes): the dense wgrad's split-K partials are
-  summed by the last-arriving CTA inside the wgrad kernel instead of by a separate k_splitk_reduce launch.  Same
-  oracle, same tolerance."""
-  ran, = _isolated([('_conv_case', (case, False))], {'RIGL_WGRAD_FIXUP': '1'})
-  assert_ran(ran, r'k_igemm_wgrad<', case)
-  assert_not_ran(ran, r'k_splitk_reduce', case)
-
-
 def test_conv_wgrad_accumulates_over_backward_passes():
-  """beta = 1: a second backward before the gradients are consumed ADDS to the dense gradient (the in-kernel
-  split-K fix-up reads dw back and adds the partials to it in split order)."""
+  """beta = 1: a second backward before the gradients are consumed ADDS to the dense gradient (k_splitk_reduce
+  reads dw back and adds the split-K partials to it in split order)."""
   pruning.reset_default_registry()
   torch.manual_seed(3)
   layer = SparseConv2d(128, 256, 3, padding='FIXED', name='acc', device=DEV)
@@ -486,15 +468,6 @@ def test_conv_cluster_multicast_64_wide_odd_m_tiles():
   cases = [(3, 8, 16, 128, 64, 1, 1, 0.5), (3, 8, 16, 64, 256, 1, 1, 0.5)]
   for case, ran in zip(cases, _isolated([('_conv_case', (c, False)) for c in cases], _MC)):
     assert_ran(ran, _KMAJOR_MC64, case)
-
-
-def test_conv_cluster_multicast_with_wgrad_fixup():
-  """RIGL_CLUSTER_MC=1 and RIGL_WGRAD_FIXUP=1 together: the split-K fix-up in the multicast wgrad kernel."""
-  cases = [CONV_CASES[8], RAGGED_CASES[3]]
-  for case, ran in zip(cases, _isolated([('_conv_case', (c, False)) for c in cases], dict(_MC, RIGL_WGRAD_FIXUP='1'))):
-    assert_ran(ran, r'k_igemm_wgrad<\d+, ?\d+, ?2>', case)
-    assert_ran(ran, _KMAJOR_MC, case)
-    assert_not_ran(ran, r'k_splitk_reduce', case)
 
 
 def _packed_layout(taps, cin, cout):
