@@ -289,7 +289,7 @@ RIGL_API int rigl_bn_forward_train(const void* y, const void* residual, const fl
                                    float* save_shift, void* out, void* ws, size_t ws_bytes, void* relu_bits,
                                    void* stream);
 /* relu_bits (optional, uint8 [rows*channels/8]): bit k of byte i <- out[8i+k] > 0.  The residual-form backward
- * needs nothing else of the block output, so it reads this bitmap (1/16 of the bytes) instead of re-reading it. */
+ * needs nothing else of the block output and requires this bitmap. */
 /* Training forward from conv-epilogue partial sums (rigl_masked_conv2d_fprop_bnstats). */
 RIGL_API int rigl_bn_forward_train_partials(const void* y, const void* residual, const float* gamma,
                                             const float* beta, const float* partial, int partial_rows,
@@ -300,23 +300,17 @@ RIGL_API int rigl_bn_forward_train_partials(const void* y, const void* residual,
 /* Inference / given statistics: out = [relu](y*scale + shift (+ residual)). */
 RIGL_API int rigl_bn_apply(const void* y, const void* residual, const float* scale, const float* shift,
                            int64_t rows, int channels, int relu, void* out, void* stream);
-/* Backward.  da = gradient of the output; y = the saved BN input; act = the saved output
- * (required only in the residual form).  dresidual != NULL selects the residual form and
- * receives the gradient of the shortcut.  Writes dy, dgamma, dbeta. */
-RIGL_API int rigl_bn_backward(const void* da, const void* y, const void* act, const float* save_mean,
-                              const float* save_rstd, const float* save_scale, const float* save_shift,
-                              int64_t rows, int channels, int relu, void* dy, void* dresidual,
-                              float* dgamma, float* dbeta, void* ws, size_t ws_bytes, void* stream);
-/* Same with the output gradient given as TWO addends, da + da2 (da2 may be NULL): the output of a
+/* Backward.  da = gradient of the output; y = the saved BN input.  dresidual != NULL selects the
+ * residual form and receives the gradient of the shortcut; that form requires relu_bits, the
+ * bitmap written by the forward pass (may be NULL otherwise).  Writes dy, dgamma, dbeta.
+ * da2 (may be NULL) is a second addend of the output gradient, residual form only: the output of a
  * residual block feeds both the next block's first conv and its shortcut, and TensorFlow's
  * gradient aggregation (an AddN per forked tensor) would otherwise be a separate elementwise pass.
- * The sum is rounded to bf16 exactly like that separate add.  Residual form only. */
-RIGL_API int rigl_bn_backward2(const void* da, const void* da2, const void* y, const void* act,
-                               const float* save_mean, const float* save_rstd, const float* save_scale,
-                               const float* save_shift, int64_t rows, int channels, int relu, void* dy,
-                               void* dresidual, float* dgamma, float* dbeta, void* ws, size_t ws_bytes,
-                               const void* relu_bits, void* stream);
-/* relu_bits: the bitmap written by the forward pass; when given, `act` is not read (may be NULL). */
+ * The sum da + da2 is rounded to bf16 exactly like that separate add. */
+RIGL_API int rigl_bn_backward(const void* da, const void* da2, const void* y, const float* save_mean,
+                              const float* save_rstd, const float* save_scale, const float* save_shift,
+                              int64_t rows, int channels, int relu, void* dy, void* dresidual, float* dgamma,
+                              float* dbeta, void* ws, size_t ws_bytes, const void* relu_bits, void* stream);
 
 /* Max pooling, NHWC bf16, TF 'SAME' padding (out = ceil(in/stride), pad_before = pad_total/2).
  * Replaces tf.layers.max_pooling2d(pool_size=3, strides=2, padding='SAME'),

@@ -92,9 +92,7 @@ SIGNATURES = {
                                                  _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'rigl_bn_apply': (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     'rigl_bn_backward': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp,
-                                   _vp, _sz, _vp]),
-    'rigl_bn_backward2': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp,
-                                    _vp, _sz, _vp, _vp]),
+                                   _vp, _sz, _vp, _vp]),
     'rigl_depthwise3x3_workspace_bytes': (_sz, [_i32, _i32, _i32, _i32, _i32]),
     'rigl_depthwise3x3_fprop': (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     'rigl_depthwise3x3_dgrad': (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),

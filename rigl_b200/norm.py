@@ -17,10 +17,6 @@ def _p(t):
   return None if t is None else t.data_ptr()
 
 
-import os as _os
-RELU_BITMASK = _os.environ.get('RIGL_BN_RELU_BITS', '1') != '0'    # 0: the residual backward re-reads the block output
-
-
 class _BNFn(torch.autograd.Function):
 
   @staticmethod
@@ -32,8 +28,8 @@ class _BNFn(torch.autograd.Function):
     save = torch.empty((4, c), dtype=torch.float32, device=dev)      # mean, rstd, scale, shift
     ws = _workspace(dev, _cabi.lib().rigl_bn_workspace_bytes(rows, c) + 8 * c + 256)
     # residual form: the backward needs only the SIGN of the block output -> one bit per element, written by the
-    # apply pass (1/16 of re-reading the bf16 tensor in the backward reduce pass)
-    bits = torch.empty(rows * c // 8, dtype=torch.uint8, device=dev) if (residual is not None and RELU_BITMASK) else None
+    # apply pass
+    bits = torch.empty(rows * c // 8, dtype=torch.uint8, device=dev) if residual is not None else None
 
     def run():
       if partial is not None:       # statistics already reduced by the producing conv's epilogue
@@ -50,19 +46,18 @@ class _BNFn(torch.autograd.Function):
           ws.numel(), _p(bits), _cabi.stream_ptr()), 'rigl_bn_forward_train')
     _timed('bn_fwd', mod, run)
     ctx.mod, ctx.has_res, ctx.fork = mod, residual is not None, bool(fork)
-    ctx.save_for_backward(y, (bits if bits is not None else out) if residual is not None else None, save)
-    ctx.has_bits = bits is not None
+    ctx.save_for_backward(y, bits, save)
     if fork:
       # Two handles on the same activation for its two consumers (next block's first conv and its
       # shortcut): backward then receives their gradients SEPARATELY and the sum is folded into
-      # the column-sum pass (rigl_bn_backward2) instead of autograd's elementwise add.
+      # the column-sum pass (rigl_bn_backward) instead of autograd's elementwise add.
       ctx.set_materialize_grads(False)
       return out, out.detach()
     return out
 
   @staticmethod
   def backward(ctx, da, da_b=None):
-    y, act, save = ctx.saved_tensors
+    y, bits, save = ctx.saved_tensors
     mod = ctx.mod
     n, c, h, w = y.shape
     rows = n * h * w
@@ -86,11 +81,10 @@ class _BNFn(torch.autograd.Function):
     ws = _workspace(y.device, _cabi.lib().rigl_bn_workspace_bytes(rows, c) + 8 * c + 256)
 
     def run():
-      _cabi.check(_cabi.lib().rigl_bn_backward2(
-          da.data_ptr(), _p(da_b), y.data_ptr(), None if ctx.has_bits else _p(act), save[0].data_ptr(),
-          save[1].data_ptr(), save[2].data_ptr(), save[3].data_ptr(), rows, c, int(mod.relu), dy.data_ptr(), _p(dres),
-          dgb[0].data_ptr(), dgb[1].data_ptr(), ws.data_ptr(), ws.numel(), _p(act) if ctx.has_bits else None,
-          _cabi.stream_ptr()), 'rigl_bn_backward2')
+      _cabi.check(_cabi.lib().rigl_bn_backward(
+          da.data_ptr(), _p(da_b), y.data_ptr(), save[0].data_ptr(), save[1].data_ptr(), save[2].data_ptr(),
+          save[3].data_ptr(), rows, c, int(mod.relu), dy.data_ptr(), _p(dres), dgb[0].data_ptr(), dgb[1].data_ptr(),
+          ws.data_ptr(), ws.numel(), _p(bits), _cabi.stream_ptr()), 'rigl_bn_backward')
     _timed('bn_bwd', mod, run)
     return dy, dgb[0], dgb[1], dres, None, None, None
 

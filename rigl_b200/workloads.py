@@ -40,7 +40,7 @@ def _BNReLU(channels, relu=True, init_zero=False, device='cuda'):
 
 
 # Block outputs are handed to their two consumers as two handles so that the gradient sum happens
-# inside the BN backward kernel (rigl_bn_backward2) rather than in a separate elementwise add.
+# inside the BN backward kernel (rigl_bn_backward) rather than in a separate elementwise add.
 FORK_BLOCK_OUTPUTS = True
 
 

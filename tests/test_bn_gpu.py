@@ -87,7 +87,7 @@ def test_bn_three_kernel_path(shape):
 @pytest.mark.parametrize('shape', [(4, 8, 8, 64), (2, 14, 14, 256), (3, 5, 9, 24)])
 def test_bn_forked_output_sums_two_gradients_in_kernel(shape):
   """fork=True hands the block output out twice; the two incoming gradients are summed inside the
-  backward column-sum pass (rigl_bn_backward2), rounded to bf16 exactly like the elementwise add
+  backward column-sum pass (rigl_bn_backward), rounded to bf16 exactly like the elementwise add
   (tf AddN / autograd accumulation) it replaces: results are bit-identical to the un-forked BN fed
   with the pre-added gradient."""
   n, h, w, c = shape
@@ -241,34 +241,33 @@ def test_conv_epilogue_bn_stats_only_where_profitable():
 
 
 @pytest.mark.parametrize('shape', [(4, 8, 8, 64), (2, 7, 7, 2048), (16, 28, 28, 128), (64, 56, 56, 64), (3, 5, 9, 24)])
-@pytest.mark.parametrize('fork', [False, True])
-def test_bn_residual_backward_relu_bitmap_equals_rereading_the_output(shape, fork):
-  """Residual form: the forward apply writes one bit per element (output > 0) and the backward reads that bitmap
-  instead of the bf16 block output (norm.RELU_BITMASK, default).  Bit-identical to re-reading the output, on the
-  3-kernel and the single-launch paths, with one or two incoming gradients."""
-  from rigl_b200 import norm
+@pytest.mark.parametrize('two_grads', [False, True])
+def test_bn_residual_relu_bitmap_is_the_sign_of_the_output(shape, two_grads):
+  """Residual form: the forward writes one bit per output element, out > 0 (k_bn_apply for C < 512, k_bn_fwd_fused
+  for C = 2048), and the backward reads nothing else of the output.  So the bitmap must be exactly the output's ReLU
+  mask; the backward, with one or two incoming gradients, runs on it."""
+  from rigl_b200 import _cabi
+  lib = _cabi.lib()
   n, h, w, c = shape
+  rows = n * h * w
   rng = np.random.RandomState(c * 3 + n)
-  y_np, r_np = rng.standard_normal(shape) * 1.3, rng.standard_normal(shape)
-  da_np, db_np = rng.standard_normal(shape), rng.standard_normal(shape)
-  res = []
-  old = norm.RELU_BITMASK
-  for use_bits in (True, False):
-    norm.RELU_BITMASK = use_bits
-    try:
-      bn = FusedBatchNormReLU(c, relu=True, device=DEV)
-      with torch.no_grad():
-        bn.weight.copy_(torch.linspace(0.5, 1.5, c))
-        bn.bias.copy_(torch.linspace(-0.3, 0.3, c))
-      y, r = _nhwc_to_dev(y_np).requires_grad_(True), _nhwc_to_dev(r_np).requires_grad_(True)
-      if fork:
-        a, b = bn(y, residual=r, fork=True)
-        torch.autograd.backward([a, b], [_nhwc_to_dev(da_np), _nhwc_to_dev(db_np)])
-      else:
-        a = bn(y, residual=r)
-        a.backward(_nhwc_to_dev(da_np))
-      res.append((a.detach().clone(), y.grad.clone(), r.grad.clone(), bn.weight.grad.clone(), bn.bias.grad.clone()))
-    finally:
-      norm.RELU_BITMASK = old
-  for got, want in zip(*res):
-    assert torch.equal(got, want)
+  y, r, da, db = (_bf(rng.standard_normal((rows, c)) * s).to(DEV) for s in (1.3, 1.0, 1.0, 1.0))
+  gamma, beta = torch.linspace(0.5, 1.5, c, device=DEV), torch.linspace(-0.3, 0.3, c, device=DEV)
+  save = torch.empty((4, c), dtype=torch.float32, device=DEV)
+  out = torch.empty_like(y)
+  bits = torch.full((rows * c // 8,), 0xFF, dtype=torch.uint8, device=DEV)
+  ws = torch.empty(lib.rigl_bn_workspace_bytes(rows, c) + 8 * c + 256, dtype=torch.uint8, device=DEV)
+  _cabi.check(lib.rigl_bn_forward_train(
+      y.data_ptr(), r.data_ptr(), gamma.data_ptr(), beta.data_ptr(), rows, c, 1e-5, 0.1, 1, None, None,
+      save[0].data_ptr(), save[1].data_ptr(), save[2].data_ptr(), save[3].data_ptr(), out.data_ptr(), ws.data_ptr(),
+      ws.numel(), bits.data_ptr(), _cabi.stream_ptr()), 'rigl_bn_forward_train')
+  want = np.packbits(out.float().cpu().numpy().reshape(-1) > 0, bitorder='little')
+  assert np.array_equal(bits.cpu().numpy(), want)
+  dy, dres = torch.empty_like(y), torch.empty_like(y)
+  dgb = torch.empty((2, c), dtype=torch.float32, device=DEV)
+  _cabi.check(lib.rigl_bn_backward(
+      da.data_ptr(), db.data_ptr() if two_grads else None, y.data_ptr(), save[0].data_ptr(), save[1].data_ptr(),
+      save[2].data_ptr(), save[3].data_ptr(), rows, c, 1, dy.data_ptr(), dres.data_ptr(), dgb[0].data_ptr(),
+      dgb[1].data_ptr(), ws.data_ptr(), ws.numel(), bits.data_ptr(), _cabi.stream_ptr()), 'rigl_bn_backward')
+  for t, what in ((dy, 'dy'), (dres, 'dresidual'), (dgb, 'dgamma/dbeta')):
+    assert torch.isfinite(t.float()).all(), what

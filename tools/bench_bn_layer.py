@@ -62,25 +62,23 @@ def main():
     save = torch.empty(4, c, device=DEV); dgb = torch.empty(2, c, device=DEV)
     ws = torch.empty(int(lib.rigl_bn_workspace_bytes(rows, c)) + 8 * c + 256, dtype=torch.uint8, device=DEV)
     p = lambda t: None if t is None else t.data_ptr()
-    use_bits = res and os.environ.get('RIGL_BN_RELU_BITS', '1') != '0'
-    bits = [torch.empty(rows * c // 8, dtype=torch.uint8, device=DEV) for _ in range(copies)] if use_bits else None
+    bits = [torch.empty(rows * c // 8, dtype=torch.uint8, device=DEV) for _ in range(copies)] if res else None
 
     def fwd(i):
       k = i % copies
       _cabi.check(lib.rigl_bn_forward_train(
           ys[k].data_ptr(), p(rs[k]) if res else None, gamma.data_ptr(), beta.data_ptr(), rows, c, 1e-5, 0.1, 1,
           rm.data_ptr(), rv.data_ptr(), save[0].data_ptr(), save[1].data_ptr(), save[2].data_ptr(),
-          save[3].data_ptr(), outs[k].data_ptr(), ws.data_ptr(), ws.numel(), bits[k].data_ptr() if use_bits else None,
+          save[3].data_ptr(), outs[k].data_ptr(), ws.data_ptr(), ws.numel(), bits[k].data_ptr() if res else None,
           _cabi.stream_ptr()), 'fwd')
 
     def bwd(i, two):
       k = i % copies
-      _cabi.check(lib.rigl_bn_backward2(
-          das[k].data_ptr(), da2s[k].data_ptr() if (res and two) else None, ys[k].data_ptr(),
-          outs[k].data_ptr() if (res and not use_bits) else None, save[0].data_ptr(), save[1].data_ptr(),
-          save[2].data_ptr(), save[3].data_ptr(), rows, c, 1, dys[k].data_ptr(), dres[k].data_ptr() if res else None,
-          dgb[0].data_ptr(), dgb[1].data_ptr(), ws.data_ptr(), ws.numel(), bits[k].data_ptr() if use_bits else None,
-          _cabi.stream_ptr()), 'bwd')
+      _cabi.check(lib.rigl_bn_backward(
+          das[k].data_ptr(), da2s[k].data_ptr() if (res and two) else None, ys[k].data_ptr(), save[0].data_ptr(),
+          save[1].data_ptr(), save[2].data_ptr(), save[3].data_ptr(), rows, c, 1, dys[k].data_ptr(),
+          dres[k].data_ptr() if res else None, dgb[0].data_ptr(), dgb[1].data_ptr(), ws.data_ptr(), ws.numel(),
+          bits[k].data_ptr() if res else None, _cabi.stream_ptr()), 'bwd')
 
     fwd(0)
     cases = [('fwd', fwd, (3 + (1 if res else 0)) * nbytes),
