@@ -202,6 +202,30 @@ RIGL_API int rigl_sgd_plan_create(const rigl_sgd_desc* params, int n_params, rig
 RIGL_API int rigl_sgd_plan_destroy(rigl_sgd_plan* plan);
 RIGL_API int rigl_sgd_plan_run(rigl_sgd_plan* plan, const float* lr_dev, float momentum, int nesterov, void* stream);
 
+/* The same for tf.train.AdamOptimizer (imagenet_train_eval.py:355-358 --use_adam, mnist_train_eval.py:247-261,
+ * rigl_tf2/utils.py get_optimizer): TF 1.x ApplyAdam, epsilon added to sqrt(v) before the bias correction.
+ *   g = (bit ? grad * grad_scale : 0) + weight_decay * w;  alpha = lr * sqrt(1 - beta2_power) / (1 - beta1_power);
+ *   m += (g - m) * (1 - beta1);  v += (g * g - v) * (1 - beta2);  w -= m * alpha / (sqrt(v) + epsilon)
+ * in float32, each operation rounded once (no FMA contraction).  lr_dev and powers_dev = {beta1_power,
+ * beta2_power} are device memory; after the update a second launch on the same stream multiplies the powers by
+ * beta1 and beta2 (TF initialises them to beta1 and beta2), so graph replays need no host work.
+ * run: 0 <= beta1, beta2 < 1, epsilon >= 0, else RIGL_ERR_INVALID_ARG before any CUDA call. */
+typedef struct {
+  float* param;                /* [n] in/out */
+  float* m;                    /* [n] in/out first moment  (TF slot 'm') */
+  float* v;                    /* [n] in/out second moment (TF slot 'v') */
+  const float* grad;           /* [n] gradient; the DENSE gradient when mask_bits != NULL */
+  const uint32_t* mask_bits;   /* NULL (dense parameter) or the layer's bitmap */
+  int64_t n;
+  float weight_decay;
+  float grad_scale;            /* multiplies grad (1/replicas for the summed dense gradients) */
+} rigl_adam_desc;
+typedef struct rigl_adam_plan rigl_adam_plan;
+RIGL_API int rigl_adam_plan_create(const rigl_adam_desc* params, int n_params, rigl_adam_plan** out);
+RIGL_API int rigl_adam_plan_destroy(rigl_adam_plan* plan);
+RIGL_API int rigl_adam_plan_run(rigl_adam_plan* plan, const float* lr_dev, float* powers_dev, float beta1, float beta2,
+                                float epsilon, void* stream);
+
 /* ------------------------------------------------------------------------
  * Masked conv2d / linear as implicit GEMM (wgmma on sm_90a; a CUDA-core
  * kernel serves shapes whose row pitch is not a 16-byte multiple).

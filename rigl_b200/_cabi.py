@@ -33,6 +33,11 @@ class SgdDesc(C.Structure):
               ('n', C.c_int64), ('weight_decay', C.c_float), ('grad_scale', C.c_float)]
 
 
+class AdamDesc(C.Structure):
+  _fields_ = [('param', C.c_void_p), ('m', C.c_void_p), ('v', C.c_void_p), ('grad', C.c_void_p),
+              ('mask_bits', C.c_void_p), ('n', C.c_int64), ('weight_decay', C.c_float), ('grad_scale', C.c_float)]
+
+
 class ConvDesc(C.Structure):
   _fields_ = [('batch', C.c_int32), ('in_h', C.c_int32), ('in_w', C.c_int32), ('cin', C.c_int32),
               ('out_h', C.c_int32), ('out_w', C.c_int32), ('cout', C.c_int32),
@@ -69,6 +74,9 @@ SIGNATURES = {
     'rigl_sgd_plan_create': (C.c_int, [C.POINTER(SgdDesc), _i32, C.POINTER(_vp)]),
     'rigl_sgd_plan_destroy': (C.c_int, [_vp]),
     'rigl_sgd_plan_run': (C.c_int, [_vp, _vp, _f32, _i32, _vp]),
+    'rigl_adam_plan_create': (C.c_int, [C.POINTER(AdamDesc), _i32, C.POINTER(_vp)]),
+    'rigl_adam_plan_destroy': (C.c_int, [_vp]),
+    'rigl_adam_plan_run': (C.c_int, [_vp, _vp, _vp, _f32, _f32, _f32, _vp]),
     'rigl_conv_workspace_bytes': (_sz, [C.POINTER(ConvDesc)]),
     'rigl_masked_conv2d_fprop': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     'rigl_bn_partial_rows': (C.c_int, []),

@@ -46,6 +46,8 @@ def variables_of(model, optimizer=None, sparse_optimizer=None, ckpt_path=None):
   parameters / buffers, (optionally) the inner optimizer's per-parameter state tensors and the sparse
   optimizer's own state.
 
+  optimizer: its slots become `<scope>/weights/<slot>`; what its `non_slot_variables()` returns (if it has
+    one) keeps its own name, e.g. `beta1_power`, `beta2_power` of optim.FusedAdam.
   sparse_optimizer: adds `last_mask_update_step` -- a non-trainable global variable in the reference
     (sparse_optimizers_base.py:166-171), so it lives in its checkpoints; without it a resumed run would
     re-initialise it to -frequency and fire an off-schedule mask update -- and, for
@@ -78,6 +80,12 @@ def variables_of(model, optimizer=None, sparse_optimizer=None, ckpt_path=None):
       for k, v in st.items():
         if hasattr(v, 'shape') and tuple(v.shape) == tuple(p.shape):
           out['%s/%s' % (names.get(id(p), 'param%d' % id(p)), k)] = _tensor_handle(v)
+    # optimizer variables that belong to no parameter (optim.FusedAdam's beta1_power / beta2_power), under
+    # TF's names; restored in place, so a captured step keeps reading them
+    non_slot = getattr(optimizer, 'non_slot_variables', None)
+    if non_slot is not None:
+      for name, v in non_slot().items():
+        out[name] = _tensor_handle(v)
   if sparse_optimizer is not None:
     so = sparse_optimizer
     out['last_mask_update_step'] = _scalar_handle(

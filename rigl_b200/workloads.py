@@ -241,20 +241,31 @@ class TrainHarness(object):
   def __init__(self, model, lr=0.1, momentum=0.9, weight_decay=1e-4, label_smoothing=0.1,
                drop_fraction=0.3, drop_fraction_anneal='cosine', begin_step=0, end_step=25000,
                frequency=100, data_parallel=None, optimizer_cls=SparseRigLOptimizer, lr_schedule=None,
-               fused_optimizer=None):
+               fused_optimizer=None, inner_optimizer='momentum'):
     """lr_schedule: optional callable(global_step) -> learning rate, evaluated on the host before every step
     (optim.make_imagenet_lr_fn is the reference's, imagenet_train_eval.py:317-354); `lr` is then only the
     initial value.  fused_optimizer: the inner optimizer is optim.FusedMomentumSGD (one launch, mask * dense_grad
-    fused in, device-resident learning rate); default on for CUDA models (RIGL_FUSED_SGD=0 -> torch.optim.SGD)."""
+    fused in, device-resident learning rate); default on for CUDA models (RIGL_FUSED_SGD=0 -> torch.optim.SGD).
+    inner_optimizer: 'momentum' (the above) or 'adam' -- optim.FusedAdam(lr, weight_decay) with TF's beta1,
+    beta2 and epsilon, the reference's `--use_adam` (imagenet_train_eval.py:355-358; there the learning rate is
+    the constant base_lr * batch / 256).  'adam' exists only on the fused path: `momentum` is then unused."""
     import os
+    if inner_optimizer not in ('momentum', 'adam'):
+      raise ValueError("inner_optimizer must be 'momentum' or 'adam', got %r" % (inner_optimizer,))
+    if inner_optimizer == 'adam' and fused_optimizer is not None and not fused_optimizer:
+      raise ValueError("inner_optimizer='adam' needs the fused optimizer: there is no non-fused Adam with "
+                       "tf.train.AdamOptimizer's arithmetic")
     self.model = model
     self.label_smoothing = label_smoothing
     self.lr_schedule = lr_schedule
     on_cuda = next(model.parameters()).is_cuda
     if fused_optimizer is None:
-      fused_optimizer = on_cuda and os.environ.get('RIGL_FUSED_SGD', '1') != '0'
+      fused_optimizer = inner_optimizer == 'adam' or (on_cuda and os.environ.get('RIGL_FUSED_SGD', '1') != '0')
     self.fused = bool(fused_optimizer)
-    if self.fused:
+    if inner_optimizer == 'adam':
+      from .optim import FusedAdam
+      self.inner = FusedAdam(model.parameters(), lr=lr, weight_decay=weight_decay)
+    elif self.fused:
       from .optim import FusedMomentumSGD
       self.inner = FusedMomentumSGD(model.parameters(), lr=lr, momentum=momentum, nesterov=True,
                                     weight_decay=weight_decay)
