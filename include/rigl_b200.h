@@ -313,7 +313,8 @@ RIGL_API int rigl_bn_forward_train(const void* y, const void* residual, const fl
                                    float* save_shift, void* out, void* ws, size_t ws_bytes, void* relu_bits,
                                    void* stream);
 /* relu_bits (optional, uint8 [rows*channels/8]): bit k of byte i <- out[8i+k] > 0.  The residual-form backward
- * needs nothing else of the block output and requires this bitmap. */
+ * with a ReLU needs nothing else of the block output and requires this bitmap; without a ReLU it carries no
+ * information and the caller passes NULL (nothing is written). */
 /* Training forward from conv-epilogue partial sums (rigl_masked_conv2d_fprop_bnstats). */
 RIGL_API int rigl_bn_forward_train_partials(const void* y, const void* residual, const float* gamma,
                                             const float* beta, const float* partial, int partial_rows,
@@ -325,12 +326,16 @@ RIGL_API int rigl_bn_forward_train_partials(const void* y, const void* residual,
 RIGL_API int rigl_bn_apply(const void* y, const void* residual, const float* scale, const float* shift,
                            int64_t rows, int channels, int relu, void* out, void* stream);
 /* Backward.  da = gradient of the output; y = the saved BN input.  dresidual != NULL selects the
- * residual form and receives the gradient of the shortcut; that form requires relu_bits, the
- * bitmap written by the forward pass (may be NULL otherwise).  Writes dy, dgamma, dbeta.
+ * residual form and receives the gradient of the shortcut; with relu != 0 that form requires relu_bits,
+ * the bitmap written by the forward pass (checked before any CUDA call); with relu == 0 relu_bits is
+ * ignored and may be NULL.  Writes dy, dgamma, dbeta.
  * da2 (may be NULL) is a second addend of the output gradient, residual form only: the output of a
  * residual block feeds both the next block's first conv and its shortcut, and TensorFlow's
  * gradient aggregation (an AddN per forked tensor) would otherwise be a separate elementwise pass.
- * The sum da + da2 is rounded to bf16 exactly like that separate add. */
+ * The sum da + da2 is rounded to bf16 exactly like that separate add.
+ * A plain no-ReLU BN whose output has two consumers (MobileNet-v2's linear bottleneck without a
+ * shortcut) uses the same call with relu == 0 and an activation-sized scratch buffer as dresidual: it
+ * receives bf16(da + da2), which the input-gradient pass then reads. */
 RIGL_API int rigl_bn_backward(const void* da, const void* da2, const void* y, const float* save_mean,
                               const float* save_rstd, const float* save_scale, const float* save_shift,
                               int64_t rows, int channels, int relu, void* dy, void* dresidual, float* dgamma,

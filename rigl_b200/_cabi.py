@@ -10,6 +10,9 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'librigl_b200.so')
 _lib = None
+# rigl_version() of the library these signatures and calling rules describe.  202: rigl_bn_backward takes the
+# residual form without a ReLU bitmap when relu == 0 (the linear bottleneck of MobileNet-v2).
+ABI_VERSION = 202
 
 
 class RiglError(RuntimeError):
@@ -123,6 +126,9 @@ def lib():
       fn = getattr(handle, name)
       fn.restype = res
       fn.argtypes = args
+    if handle.rigl_version() < ABI_VERSION:
+      raise RiglError('librigl_b200.so is older (rigl_version %d) than this package needs (%d): rebuild with '
+                      '`python -m rigl_b200.build`' % (handle.rigl_version(), ABI_VERSION))
     _lib = handle
   return _lib
 

@@ -10,6 +10,9 @@
 //   backward: reduce : read da, y (, ReLU bits)   -> dbeta = sum g, dgamma = sum g*xhat  (g = da * relu')
 //                      (residual form also writes g, which IS the gradient of the shortcut)
 //             apply  : read g|da, y               -> dy = scale * (g - dbeta/M - xhat*dgamma/M)
+// MobileNet-v2's linear bottleneck (rigl/imagenet_resnet/mobilenetv2_model.py:246-252) is a BN WITHOUT ReLU, with or
+// without an identity shortcut, whose output may have two consumers.  Its residual form stores no ReLU bitmap and its
+// backward (column-sum MODE 3) never loads one; a forked plain no-ReLU BN reuses that form with a scratch g.
 // Every kernel moves 16-byte vectors (8 channels) per thread with the channel dimension
 // innermost, so global traffic is fully coalesced; reductions go registers -> smem ->
 // per-block partials -> a tiny finalize kernel (fixed order: deterministic).
@@ -54,12 +57,14 @@ __host__ __device__ __forceinline__ RowGroup row_group(int C, int threads) {
 // MODE 0: (y, y^2)                                   -> forward statistics
 // MODE 1: (g, g*xhat), g = da * [fma(y,scale,shift) > 0 if relu]      (plain BN / BN+ReLU)
 // MODE 2: (g, g*xhat), g = (da [+ da2]) * [relu_bits if relu], g written to gout    (residual form)
+// MODE 3: (g, g*xhat), g = da [+ da2], g written to gout     (residual form without ReLU, or a plain no-ReLU BN
+//         whose output has two consumers: the linear bottleneck of MobileNet-v2).  Never touches relu_bits.
 // partial[block][2][C] fp32.
 template <int MODE, int THREADS>
 __device__ __forceinline__ void colsum_rows(
     const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ da,
     const __nv_bfloat16* __restrict__ da2 /* MODE 2: optional second addend of the output gradient */,
-    const uint8_t* __restrict__ relu_bits /* MODE 2: bit k of byte i <- forward output [8i+k] > 0 */,
+    const uint8_t* __restrict__ relu_bits /* MODE 2 only: bit k of byte i <- forward output [8i+k] > 0 */,
     __nv_bfloat16* __restrict__ gout, const float* __restrict__ mean, const float* __restrict__ rstd,
     const float* __restrict__ scale, const float* __restrict__ shift, int relu, long long row0, long long row1,
     int C, float* __restrict__ partial_row /* [2][C] */, float* red /* smem [rpi][vl][16] */) {
@@ -93,10 +98,8 @@ __device__ __forceinline__ void colsum_rows(
             const long long off = r * C + 8 * v;
             qy[u] = *reinterpret_cast<const uint4*>(y + off);
             if (MODE != 0) qd[u] = *reinterpret_cast<const uint4*>(da + off);
-            if (MODE == 2) {
-              qb[u] = relu_bits[off >> 3];
-              if (da2) qe[u] = *reinterpret_cast<const uint4*>(da2 + off);
-            }
+            if (MODE == 2) qb[u] = relu_bits[off >> 3];
+            if (MODE >= 2 && da2) qe[u] = *reinterpret_cast<const uint4*>(da2 + off);
           }
         }
 #pragma unroll
@@ -111,15 +114,17 @@ __device__ __forceinline__ void colsum_rows(
           } else {
             float g[8];
             unpack8(qd[u], g);
-            if (MODE == 2) {
+            if (MODE >= 2) {
               if (da2) {       // the block output feeds two consumers: their gradients are summed here
                 float g2[8];   // (rounded to bf16 like the separate elementwise add it replaces)
                 unpack8(qe[u], g2);
 #pragma unroll
                 for (int i = 0; i < 8; ++i) g[i] = __bfloat162float(__float2bfloat16(g[i] + g2[i]));
               }
+              if (MODE == 2) {
 #pragma unroll
-              for (int i = 0; i < 8; ++i) g[i] = (!relu || ((qb[u] >> i) & 1u)) ? g[i] : 0.f;
+                for (int i = 0; i < 8; ++i) g[i] = (!relu || ((qb[u] >> i) & 1u)) ? g[i] : 0.f;
+              }
               *reinterpret_cast<uint4*>(gout + off) = pack8(g);
             } else if (relu) {
 #pragma unroll
@@ -518,7 +523,7 @@ k_bn_bwd_fused(const __nv_bfloat16* __restrict__ da, const __nv_bfloat16* __rest
     const int V = C >> 3;
     const long long i_end = row1 * V;
     const bool fixed_v = (kFusedThreads % V) == 0;
-    const __nv_bfloat16* g_src = (MODE == 2) ? gout : da;      // (gout was written by THIS CTA for these rows)
+    const __nv_bfloat16* g_src = (MODE >= 2) ? gout : da;      // (gout was written by THIS CTA for these rows)
     float sc[8], sh[8], P[8], Q[8];
     long long i = row0 * V + threadIdx.x;
     auto load_coef = [&](int v) {
@@ -559,7 +564,7 @@ k_bn_bwd_fused(const __nv_bfloat16* __restrict__ da, const __nv_bfloat16* __rest
 static bool g_bn_fused = true;            // RIGL_BN_FUSED=0: always the 3-kernel path
 static size_t g_bn_fused_max_bytes = (size_t)64 << 20;
 static BnSync* g_bn_sync[16] = {};
-static int g_bn_fused_grid[3] = {0, 0, 0};   // co-resident CTAs: fwd, bwd<1>, bwd<2> (0 = not probed)
+static int g_bn_fused_grid[4] = {0, 0, 0, 0};   // co-resident CTAs: fwd, bwd<1>, bwd<2>, bwd<3> (0 = not probed)
 
 // Dynamic shared memory of the column-sum pass: [rpi][vl][16] floats.
 static size_t colsum_smem(int C, int threads) {
@@ -596,15 +601,16 @@ static int fused_plan(int which, long long rows, int C, long long* rows_per_blk,
     cudaError_t e = cudaSuccess;
     if (which == 0) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bn_fwd_fused, kFusedThreads, 32 * 1024);
     else if (which == 1) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bn_bwd_fused<1>, kFusedThreads, 32 * 1024);
-    else e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bn_bwd_fused<2>, kFusedThreads, 32 * 1024);
+    else if (which == 2) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bn_bwd_fused<2>, kFusedThreads, 32 * 1024);
+    else e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bn_bwd_fused<3>, kFusedThreads, 32 * 1024);
     if (e != cudaSuccess || per_sm < 1) { g_bn_fused_grid[which] = -1; return 0; }
     if (per_sm > 2) per_sm = 2;
     g_bn_fused_grid[which] = sms * per_sm;
   }
   if (g_bn_fused_grid[which] < 0) return 0;
   if (g_bn_sync[dev] == nullptr) {
-    if (cudaMalloc(&g_bn_sync[dev], 3 * sizeof(BnSync)) != cudaSuccess) return 0;
-    cudaMemset(g_bn_sync[dev], 0, 3 * sizeof(BnSync));
+    if (cudaMalloc(&g_bn_sync[dev], 4 * sizeof(BnSync)) != cudaSuccess) return 0;
+    cudaMemset(g_bn_sync[dev], 0, 4 * sizeof(BnSync));
   }
   const long long rpb = rows_per_block(rows, C, kFusedThreads, g_bn_fused_grid[which]);
   *rows_per_blk = rpb;
@@ -721,22 +727,29 @@ extern "C" int rigl_bn_backward(const void* da, const void* da2, const void* y, 
   RIGL_REQUIRE(da && y && save_mean && save_rstd && save_scale && save_shift && dy && dgamma && dbeta && ws,
                "rigl_bn_backward: null argument");
   RIGL_REQUIRE(rows > 0 && channels > 0 && channels % 8 == 0, "rigl_bn_backward: channels must be a multiple of 8");
-  RIGL_REQUIRE(dresidual == nullptr || relu_bits != nullptr,
-               "rigl_bn_backward: the residual form needs the ReLU bitmap written by the forward pass");
+  RIGL_REQUIRE(dresidual == nullptr || !relu || relu_bits != nullptr,
+               "rigl_bn_backward: the residual form with a ReLU needs the ReLU bitmap written by the forward pass");
   cudaStream_t s = (cudaStream_t)stream_;
   const bool residual_form = dresidual != nullptr;
+  // 1: plain (da, recomputed ReLU mask); 2: residual with ReLU (stored bitmap); 3: residual / forked without ReLU
+  const int mode = !residual_form ? 1 : relu ? 2 : 3;
   {
     BnSync* sync = nullptr;
     long long frpb;
-    const int grid = fused_plan(residual_form ? 2 : 1, rows, channels, &frpb, &sync);
+    const int grid = fused_plan(mode, rows, channels, &frpb, &sync);
     if (grid > 0 && ws_bytes >= ((size_t)grid * 2 * channels + 2 * channels) * sizeof(float)) {
       float* partial = static_cast<float*>(ws);
       float* coef = partial + (size_t)grid * 2 * channels;
-      if (residual_form) {
+      if (mode == 2) {
         k_bn_bwd_fused<2><<<grid, kFusedThreads, colsum_smem(channels, kFusedThreads), s>>>(
             (const __nv_bfloat16*)da, (const __nv_bfloat16*)da2, (const __nv_bfloat16*)y,
             static_cast<const uint8_t*>(relu_bits), save_mean, save_rstd, save_scale, save_shift, rows, channels, frpb,
             relu, (__nv_bfloat16*)dy, (__nv_bfloat16*)dresidual, dgamma, dbeta, partial, coef, sync);
+      } else if (mode == 3) {
+        k_bn_bwd_fused<3><<<grid, kFusedThreads, colsum_smem(channels, kFusedThreads), s>>>(
+            (const __nv_bfloat16*)da, (const __nv_bfloat16*)da2, (const __nv_bfloat16*)y, nullptr, save_mean,
+            save_rstd, save_scale, save_shift, rows, channels, frpb, 0, (__nv_bfloat16*)dy, (__nv_bfloat16*)dresidual,
+            dgamma, dbeta, partial, coef, sync);
       } else {
         k_bn_bwd_fused<1><<<grid, kFusedThreads, colsum_smem(channels, kFusedThreads), s>>>(
             (const __nv_bfloat16*)da, nullptr, (const __nv_bfloat16*)y, nullptr, save_mean, save_rstd, save_scale,
@@ -755,12 +768,17 @@ extern "C" int rigl_bn_backward(const void* da, const void* da2, const void* y, 
   }
   float* partial = static_cast<float*>(ws);
   float* coef = partial + (size_t)nb * 2 * channels;
-  if (residual_form) {
+  if (mode == 2) {
     k_bn_colsum<2><<<nb, kBnThreads, colsum_smem(channels, kBnThreads), s>>>(
         (const __nv_bfloat16*)y, (const __nv_bfloat16*)da, (const __nv_bfloat16*)da2,
         static_cast<const uint8_t*>(relu_bits), (__nv_bfloat16*)dresidual, save_mean, save_rstd, save_scale,
         save_shift, relu, rows, channels, rpb, partial);
     RIGL_LAUNCH_CHECK("k_bn_colsum<2>");
+  } else if (mode == 3) {
+    k_bn_colsum<3><<<nb, kBnThreads, colsum_smem(channels, kBnThreads), s>>>(
+        (const __nv_bfloat16*)y, (const __nv_bfloat16*)da, (const __nv_bfloat16*)da2, nullptr,
+        (__nv_bfloat16*)dresidual, save_mean, save_rstd, save_scale, save_shift, 0, rows, channels, rpb, partial);
+    RIGL_LAUNCH_CHECK("k_bn_colsum<3>");
   } else {
     k_bn_colsum<1><<<nb, kBnThreads, colsum_smem(channels, kBnThreads), s>>>(
         (const __nv_bfloat16*)y, (const __nv_bfloat16*)da, nullptr, nullptr, nullptr, save_mean, save_rstd, save_scale,

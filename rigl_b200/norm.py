@@ -27,9 +27,9 @@ class _BNFn(torch.autograd.Function):
     out = torch.empty_like(y, memory_format=torch.channels_last)
     save = torch.empty((4, c), dtype=torch.float32, device=dev)      # mean, rstd, scale, shift
     ws = _workspace(dev, _cabi.lib().rigl_bn_workspace_bytes(rows, c) + 8 * c + 256)
-    # residual form: the backward needs only the SIGN of the block output -> one bit per element, written by the
-    # apply pass
-    bits = torch.empty(rows * c // 8, dtype=torch.uint8, device=dev) if residual is not None else None
+    # residual form with a ReLU: the backward needs only the SIGN of the block output -> one bit per element,
+    # written by the apply pass.  Without a ReLU (MobileNet-v2's linear bottleneck) the backward needs nothing of it.
+    bits = torch.empty(rows * c // 8, dtype=torch.uint8, device=dev) if (residual is not None and mod.relu) else None
 
     def run():
       if partial is not None:       # statistics already reduced by the producing conv's epilogue
@@ -73,17 +73,30 @@ class _BNFn(torch.autograd.Function):
     da = as_grad(da)
     if da_b is not None:
       da_b = as_grad(da_b)
-      if not ctx.has_res:           # only the residual form sums in-kernel
+      if not ctx.has_res and mod.relu:       # a forked plain BN+ReLU: the sum is a separate elementwise add
         da, da_b = da + da_b, None
     dy = torch.empty_like(y, memory_format=torch.channels_last)
-    dres = torch.empty_like(y, memory_format=torch.channels_last) if ctx.has_res else None
+    # What the kernel writes besides dy (`g_out`, its residual-form output) and what this returns as the
+    # gradient of the shortcut:
+    #   residual, ReLU              g = da [+ da_b] masked by the bitmap -> a new tensor, returned
+    #   residual, no ReLU, 1 grad   g = da itself: the plain form runs and `da` is handed back, no copy
+    #   residual, no ReLU, 2 grads  g = bf16(da + da_b)                  -> a new tensor, returned
+    #   plain, no ReLU, 2 grads     g = bf16(da + da_b)                  -> scratch that the dy pass reads (one
+    #                               pass fewer than the elementwise add + plain backward: 7 vs 8 tensor passes)
+    g_out, dres = None, None
+    if ctx.has_res and (mod.relu or da_b is not None):
+      g_out = dres = torch.empty_like(y, memory_format=torch.channels_last)
+    elif ctx.has_res:
+      dres = da
+    elif da_b is not None:
+      g_out = torch.empty_like(y, memory_format=torch.channels_last)
     dgb = torch.empty((2, c), dtype=torch.float32, device=y.device)
     ws = _workspace(y.device, _cabi.lib().rigl_bn_workspace_bytes(rows, c) + 8 * c + 256)
 
     def run():
       _cabi.check(_cabi.lib().rigl_bn_backward(
           da.data_ptr(), _p(da_b), y.data_ptr(), save[0].data_ptr(), save[1].data_ptr(), save[2].data_ptr(),
-          save[3].data_ptr(), rows, c, int(mod.relu), dy.data_ptr(), _p(dres), dgb[0].data_ptr(), dgb[1].data_ptr(),
+          save[3].data_ptr(), rows, c, int(mod.relu), dy.data_ptr(), _p(g_out), dgb[0].data_ptr(), dgb[1].data_ptr(),
           ws.data_ptr(), ws.numel(), _p(bits), _cabi.stream_ptr()), 'rigl_bn_backward')
     _timed('bn_bwd', mod, run)
     return dy, dgb[0], dgb[1], dres, None, None, None
@@ -108,7 +121,8 @@ class FusedBatchNormReLU(nn.Module):
     """`producer`: the SparseConv2d whose output `y` is; if its epilogue emitted the batch statistics
     of exactly this tensor (layer.bn_partial), the stats pass is skipped.
     `fork`: return the activation TWICE (same storage) for its two consumers; their gradients are
-    then summed inside the backward kernel instead of by a separate elementwise add."""
+    then summed inside the backward kernel instead of by a separate elementwise add (residual form, and
+    the plain form without ReLU)."""
     if y.dim() != 4 or y.shape[1] != self.channels:
       raise ValueError('expected [N,%d,H,W]' % self.channels)
     partial = None

@@ -6,9 +6,12 @@ that the masked conv/linear kernels and the RigL update run on:
   ResNet50   rigl/imagenet_resnet/resnet_model.py:396-731 (v1.5: stride on the 3x3;
              BN after every conv, zero-init gamma on the last BN of a block)
   MnistFC    rigl/mnist/mnist_train_eval.py:112-160 (784-300-100-10, all masked)
+  MobileNetV2 rigl/imagenet_resnet/mobilenetv2_model.py (inverted residual blocks, linear bottlenecks)
 BN+ReLU(+residual) run on the fused streaming kernels of csrc/bn.cu (SURVEY 8f row 1);
 pooling / loss are stock PyTorch kernels over channels_last bf16 tensors.
 """
+import math
+
 import numpy as np
 import torch
 from torch import nn
@@ -202,6 +205,128 @@ class MobileNetV1(nn.Module):
       x = blk.bn_dw(blk.depthwise(x))
       x = blk.bn_pw(blk.pointwise(x))
     return self.final_dense(x.mean(dim=(2, 3)))
+
+
+def _make_divisible(v, divisor=8, min_value=None):
+  """mobilenetv2_model.py:33-40: round to a multiple of `divisor`, never more than 10 % down."""
+  if min_value is None:
+    min_value = divisor
+  new_v = max(min_value, int(v + divisor / 2) // divisor * divisor)
+  if new_v < 0.9 * v:
+    new_v += divisor
+  return new_v
+
+
+def _trunc_variance_scaling_(t, fan_in):
+  """tf.variance_scaling_initializer() defaults: scale 1, fan_in, truncated normal (|z| <= 2 sigma, the
+  untruncated standard deviation divided by 0.8796... so the truncated one is sqrt(1 / fan_in))."""
+  std = math.sqrt(1.0 / max(fan_in, 1)) / .87962566103423978
+  with torch.no_grad():
+    nn.init.trunc_normal_(t, 0., std, -2. * std, 2. * std)
+  return t
+
+
+def _hwio_init(w):
+  return _trunc_variance_scaling_(w, int(np.prod(w.shape[:-1])))
+
+
+# (filters, stride) of inverted_res_block 0..16, mobilenetv2_model.py:318-340
+MOBILENET_V2_BLOCKS = ((16, 1), (24, 2), (24, 1), (32, 2), (32, 1), (32, 1), (64, 2), (64, 1), (64, 1), (64, 1),
+                       (96, 1), (96, 1), (96, 1), (160, 2), (160, 1), (160, 1), (320, 1))
+
+
+def mobilenet_v2_plan(width=1.0, expansion_factor=6.0):
+  """Channel plan of mobilenet_v2_generator: (initial_conv filters, [(block_id, cin, expanded width or None,
+  stride, cout, identity shortcut)], final_1x1_conv filters).  Every width must be a multiple of 8 (the NHWC
+  kernels move 8 channels per 16-byte vector); ValueError names the first layer that is not."""
+  def need8(c, layer):
+    if c % 8:
+      raise ValueError('MobileNetV2(width=%g, expansion_factor=%g): %s has %d channels, not a multiple of 8'
+                       % (width, expansion_factor, layer, c))
+    return c
+  c0 = need8(_make_divisible(32 * width), 'initial_conv')
+  blocks, prev = [], c0
+  for b, (filters, stride) in enumerate(MOBILENET_V2_BLOCKS):
+    expand = need8(int(expansion_factor * prev), 'expand_1x1_%d' % b) if b else None
+    cout = need8(_make_divisible(int(width * filters), divisor=8 if b else 1), 'contraction_1x1_%d' % b)
+    blocks.append((b, prev, expand, stride, cout, prev == cout and stride == 1))
+    prev = cout
+  last = need8(max(1280, _make_divisible(1280 * width, 8)), 'final_1x1_conv')
+  return c0, blocks, last
+
+
+class MobileNetV2(nn.Module):
+  """MobileNet-v2 as mobilenetv2_model.py:156-398 builds it: plain ReLU (not ReLU6); the masked 1x1 convs
+  `expand_1x1_{1..16}`, `contraction_1x1_{0..16}`, `final_1x1_conv` and (prune_last_layer) `final_dense`; dense
+  `initial_conv` (3x3/2, 32 * width channels) and depthwise 3x3 convs, fixed padding where strided.  The
+  contraction BN has no ReLU ("linear bottleneck"); where the block keeps its depth at stride 1 the input is
+  added after it, with no activation after the add (fused into the BN kernel, csrc/bn.cu).  Block outputs whose
+  next block has an identity shortcut are handed on as two handles (fork), as in ResNet50."""
+
+  def __init__(self, num_classes=1000, width=1.0, expansion_factor=6.0, prune_last_layer=True, device='cuda',
+               registry=None):
+    super(MobileNetV2, self).__init__()
+    c0, plan, last = mobilenet_v2_plan(width, expansion_factor)     # (raises before any parameter exists)
+    self.registry = registry if registry is not None else pruning.MaskedLayerRegistry()
+    reg = self.registry
+
+    def mk(ci, co, n):
+      conv = SparseConv2d(ci, co, 1, strides=1, padding='FIXED', name='resnet_model/' + n, device=device,
+                          registry=reg, kernel_initializer=_hwio_init)
+      conv.collect_bn_stats = True        # the epilogue emits the BN statistics where that pays (conv heuristic)
+      return conv
+    self.initial_conv = DenseConv2d(3, c0, 3, stride=2, padding=1, bias=False, device=device)
+    _trunc_variance_scaling_(self.initial_conv.weight, 27)
+    self.initial_bn = _BNReLU(c0, device=device)
+    blocks = []
+    for b, cin, expand, stride, cout, shortcut in plan:
+      blk = nn.Module()
+      blk.shortcut = shortcut
+      blk.expand = None
+      mid = cin
+      if expand is not None:
+        blk.expand = mk(cin, expand, 'expand_1x1_%d' % b)
+        blk.bn_expand = _BNReLU(expand, device=device)
+        mid = expand
+      blk.depthwise = DepthwiseConv2d(mid, stride=stride, device=device)
+      # contrib separable_conv2d's default xavier (glorot uniform) init on the [3,3,C,1] depthwise kernel
+      bound = math.sqrt(6.0 / (9 * mid + 9))
+      with torch.no_grad():
+        blk.depthwise.weight.uniform_(-bound, bound)
+      blk.bn_dw = _BNReLU(mid, device=device)
+      blk.contraction = mk(mid, cout, 'contraction_1x1_%d' % b)
+      blk.bn_contraction = _BNReLU(cout, relu=False, device=device)
+      blocks.append(blk)
+    self.blocks = nn.ModuleList(blocks)
+    self.final_conv = mk(plan[-1][4], last, 'final_1x1_conv')
+    self.final_bn = _BNReLU(last, device=device)
+    self.prune_last_layer = bool(prune_last_layer)
+    if self.prune_last_layer:
+      self.final_dense = SparseLinear(last, num_classes, name='resnet_model/final_dense', device=device, registry=reg,
+                                      out_dtype=torch.float32, kernel_initializer=_hwio_init)
+    else:             # tf.layers.dense: not masked, fp32
+      self.final_dense = nn.Linear(last, num_classes, device=device)
+      with torch.no_grad():
+        _trunc_variance_scaling_(self.final_dense.weight, last)
+        self.final_dense.bias.zero_()
+
+  def forward(self, x):
+    x = self.initial_bn(self.initial_conv(x.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)))
+    x_skip = x
+    for i, blk in enumerate(self.blocks):
+      h = x
+      if blk.expand is not None:
+        h = blk.bn_expand(blk.expand(h), producer=blk.expand)
+      h = blk.bn_dw(blk.depthwise(h))
+      fork = FORK_BLOCK_OUTPUTS and i + 1 < len(self.blocks) and self.blocks[i + 1].shortcut
+      y = blk.bn_contraction(blk.contraction(h), residual=x_skip if blk.shortcut else None,
+                             producer=blk.contraction, fork=fork)
+      x, x_skip = y if fork else (y, y)
+    x = self.final_bn(self.final_conv(x), producer=self.final_conv)
+    x = x.mean(dim=(2, 3))
+    if not self.prune_last_layer:
+      x = x.float()
+    return self.final_dense(x)
 
 
 class MnistFC(nn.Module):
