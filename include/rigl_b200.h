@@ -263,6 +263,17 @@ RIGL_API int rigl_masked_conv2d_fprop_bnstats(const rigl_conv_desc* d, const voi
  * <= 128 output channels; otherwise RIGL_ERR_UNSUPPORTED and the caller runs the plain call + a stats pass).
  * on != 0: for every supported shape (tests). */
 RIGL_API int rigl_set_bn_stats_always(int on);
+/* Inference fprop with the batch norm applied in the conv epilogue:
+ *   y = [relu](bf16(conv(x, mask*W)) * scale[c] + shift[c] (+ residual)), rounded to bf16,
+ * bit-identical to rigl_masked_conv2d_fprop followed by rigl_bn_apply on the same coefficients, without writing
+ * and re-reading the conv output.  residual (may be NULL) is bf16 NHWC in y's layout; scale / shift are fp32
+ * [cout]; cout % 8 == 0; x, y and residual 16-byte aligned (checked before any CUDA call).  Only layers on the
+ * K-major tensor-core kernel with the TMA-store epilogue have the variant: halo-eligible 3x3 layers, the
+ * 3-channel stem, the CUDA-core path (RIGL_FORCE_SIMT=1) and RIGL_TMA_STORE=0 return RIGL_ERR_UNSUPPORTED and
+ * launch nothing; the caller then runs the plain fprop + rigl_bn_apply. */
+RIGL_API int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const void* x, const void* packed,
+                                              const void* residual, const float* scale, const float* shift, int relu,
+                                              void* y_bf16, void* ws, size_t ws_bytes, void* stream);
 /* dx = conv^T(dy, mask*W). */
 RIGL_API int rigl_masked_conv2d_dgrad(const rigl_conv_desc* d, const void* dy, const void* packed,
                                       void* dx, void* ws, size_t ws_bytes, void* stream);

@@ -11,7 +11,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'librigl_b200.so')
 _lib = None
 # rigl_version() of the library these signatures and calling rules describe.  202: rigl_bn_backward takes the
-# residual form without a ReLU bitmap when relu == 0 (the linear bottleneck of MobileNet-v2).
+# residual form without a ReLU bitmap when relu == 0 (the linear bottleneck of MobileNet-v2).  Library version 203
+# only adds rigl_masked_conv2d_fprop_bnapply; no calling rule of an existing symbol changed, and a library without
+# the new symbol already fails its lookup in lib().
 ABI_VERSION = 202
 
 
@@ -85,6 +87,8 @@ SIGNATURES = {
     'rigl_bn_partial_rows': (C.c_int, []),
     'rigl_set_bn_stats_always': (C.c_int, [_i32]),
     'rigl_masked_conv2d_fprop_bnstats': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, C.POINTER(C.c_int), _vp, _sz, _vp]),
+    'rigl_masked_conv2d_fprop_bnapply': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _sz,
+                                                   _vp]),
     'rigl_masked_conv2d_dgrad': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _sz, _vp]),
     'rigl_conv2d_wgrad_dense': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _f32, _vp, _sz, _vp]),
     'rigl_im2col_nhwc': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _i64, _vp]),

@@ -148,6 +148,24 @@ extern "C" int rigl_masked_conv2d_fprop_bnstats(const rigl_conv_desc* d, const v
   return tc_fprop(g, x, packed, y_bf16, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream, bn_partial, bn_rows_out);
 }
 
+extern "C" int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const void* x, const void* packed,
+                                                const void* residual, const float* scale, const float* shift, int relu,
+                                                void* y_bf16, void* ws, size_t ws_bytes, void* stream) {
+  ConvGeom g;
+  int rc = geom_from_desc(d, &g);
+  if (rc != RIGL_OK) return rc;
+  RIGL_REQUIRE(x && packed && scale && shift && y_bf16, "rigl_masked_conv2d_fprop_bnapply: null argument");
+  RIGL_REQUIRE(g.cout % 8 == 0, "rigl_masked_conv2d_fprop_bnapply: cout %d is not a multiple of 8", g.cout);
+  RIGL_REQUIRE(aligned16(x) && aligned16(y_bf16) && aligned16(residual),
+               "rigl_masked_conv2d_fprop_bnapply: tensors must be 16-byte aligned");
+  if (force_simt() || !tc_supported(g, 0)) {    // (this includes the 3-channel stem)
+    set_error("rigl_masked_conv2d_fprop_bnapply: shape not on the K-major tensor-core kernel");
+    return RIGL_ERR_UNSUPPORTED;
+  }
+  const BnApplyArgs bn = {residual, scale, shift, relu};
+  return tc_fprop(g, x, packed, y_bf16, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream, nullptr, nullptr, &bn);
+}
+
 extern "C" int rigl_masked_conv2d_dgrad(const rigl_conv_desc* d, const void* dy, const void* packed,
                                         void* dx, void* ws, size_t ws_bytes, void* stream) {
   ConvGeom g;

@@ -51,12 +51,22 @@ int simt_dgrad(const ConvGeom& g, const void* dy, const void* w_fprop, void* dx,
 int simt_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float beta, cudaStream_t s);
 int simt_im2col(const ConvGeom& g, const void* x, void* out, int64_t out_pitch, cudaStream_t s);
 
+// Inference batch norm applied by the K-major fprop epilogue (rigl_masked_conv2d_fprop_bnapply):
+// y = [relu](conv * scale + shift [+ residual]), residual bf16 in y's layout or null.
+struct BnApplyArgs {
+  const void* residual;
+  const float* scale;
+  const float* shift;
+  int relu;
+};
+
 // tensor-core path (igemm_tc.cu)
 bool tc_supported(const ConvGeom& g, int which /*0 fprop, 1 dgrad, 2 wgrad*/);
 size_t tc_workspace_bytes(const ConvGeom& g);
+// bn_apply != null: RIGL_ERR_UNSUPPORTED unless the layer runs on k_igemm_kmajor with the TMA-store epilogue.
 int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32,
              const float* bias, void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial = nullptr,
-             int* bn_rows = nullptr);
+             int* bn_rows = nullptr, const BnApplyArgs* bn_apply = nullptr);
 int tc_max_ctas();
 void tc_set_bn_stats_always(bool on);
 int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, void* ws,

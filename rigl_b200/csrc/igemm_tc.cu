@@ -73,6 +73,14 @@ struct IgemmParams {
   float* bn_partial;                // optional [gridDim.x][2][N]: per-CTA column sums / sums of squares of D
 };
 
+// Inference batch norm applied by the epilogue of k_igemm_kmajor_bn (TMA-store path only).
+struct BnEpilogue {
+  const float* scale;               // [N]
+  const float* shift;               // [N]
+  int relu;
+  int residual;                     // 1: the residual box is TMA-loaded into the staging slab before it is staged
+};
+
 struct TMaps4 {
   CUtensorMap a[4];
 };
@@ -171,6 +179,44 @@ __device__ __forceinline__ void stage_slab(const float (&d)[R], uint32_t slab, i
   }
 }
 
+// stage_slab with the inference batch norm applied: each stored pair is
+//   [relu](fmaf(float(bf16_rn(D)), scale[c], shift[c]) [+ residual]) rounded to bf16,
+// the arithmetic of bn.cu's bn_apply8 on exactly the value stage_slab would store, so the result is bit-identical
+// to the plain fprop followed by rigl_bn_apply.  With `has_res` the slab already holds the residual box (TMA-loaded
+// in the store's layout): every thread reads the words it is about to overwrite, and no other thread touches them.
+// Coefficients of channels >= n (a ragged last slab) are not read; those columns are clipped by the store.
+template <int S, int R>
+__device__ __forceinline__ void stage_slab_bn(const float (&d)[R], uint32_t slab, int row, bool ok0, bool ok1, int lane,
+                                              const BnEpilogue& ep, int co0, int n) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+    const int co = co0 + 8 * jj + 2 * (lane & 3);
+    float sc0 = 0.f, sc1 = 0.f, sh0 = 0.f, sh1 = 0.f;
+    if (co < n) {                  // (n is a multiple of 8, so co + 1 < n as well)
+      sc0 = __ldg(ep.scale + co); sc1 = __ldg(ep.scale + co + 1);
+      sh0 = __ldg(ep.shift + co); sh1 = __ldg(ep.shift + co + 1);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row + 8 * h;
+      const int e = 4 * (8 * S + jj) + 2 * h;
+      const uint32_t dst = slab + (uint32_t)r * 128u + (uint32_t)((jj ^ (r & 7)) << 4) + (uint32_t)(lane & 3) * 4u;
+      const float2 f = __bfloat1622float2(__floats2bfloat162_rn(d[e], d[e + 1]));
+      float a = fmaf(f.x, sc0, sh0), b = fmaf(f.y, sc1, sh1);
+      if (ep.residual) {
+        uint32_t rw;
+        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rw) : "r"(dst) : "memory");
+        a += __uint_as_float(rw << 16);
+        b += __uint_as_float(rw & 0xffff0000u);
+      }
+      if (ep.relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+      __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+      const uint32_t w = (h ? ok1 : ok0) ? *reinterpret_cast<uint32_t*>(&v) : 0u;
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(w) : "memory");
+    }
+  }
+}
+
 template <int R>
 __device__ __forceinline__ void zero_acc(float (&d)[R]) {
 #pragma unroll
@@ -199,10 +245,11 @@ __device__ __forceinline__ void release_stage(uint32_t bar) {
 // CL = CTAs per cluster (1 or 2).  With CL == 2 the two CTAs work on the two M tiles of a tile PAIR that share the
 // weight tile: each loads HALF of B and multicasts it into both CTAs' shared memory.  A stage is refilled only when
 // the consumers of BOTH CTAs have released it: every consumer warp arrives on the empty barrier of each CTA.
-template <int BN, int STAGES, int CL>
-__global__ void __launch_bounds__(kThreads, 1)
-k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
-               const __grid_constant__ CUtensorMap omap, const IgemmParams p) {
+// kBnApply: the epilogue applies the inference batch norm (stage_slab_bn) and, with ep.residual, first TMA-loads the
+// residual box at the output tile's coordinates into the staging slab (one more mbarrier, no more shared memory).
+template <int BN, int STAGES, int CL, bool kBnApply>
+__device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
+                                            const IgemmParams& p, const CUtensorMap* rmap, const BnEpilogue& ep) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr uint32_t kABytes = kBM * kBK * 2;        // 16 KB
   constexpr uint32_t kBBytes = BN * kBK * 2;
@@ -213,6 +260,7 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
   const uint32_t bar_base = out_base + 2 * kSlabBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  const uint32_t res_bar = bar_base + 8u * (2 * STAGES);             // kBnApply: residual box loaded
 
   // live_cons[warpgroup][tile parity]: one liveness mask per consumer warpgroup, double-buffered over tiles
   __shared__ uint32_t live_prod[kLiveWords], live_cons[2][2][kLiveWords];
@@ -222,6 +270,10 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
     prefetch_tmap(&bmap);
     if (p.tma_store) prefetch_tmap(&omap);
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps * CL); }
+    if constexpr (kBnApply) {
+      mbar_init(res_bar, 1);
+      if (ep.residual) prefetch_tmap(rmap);
+    }
     fence_barrier_init();
   }
   if (CL > 1) cluster_sync_all(); else __syncthreads();     // peers' barriers are live before any multicast
@@ -278,7 +330,8 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
     float acc[BN / 2];
     int stage = 0; uint32_t phase = 0;
     uint32_t slab_ctr = 0;
-    float* bn_row = p.bn_partial ? p.bn_partial + (size_t)blockIdx.x * 2 * p.N : nullptr;
+    uint32_t res_phase = 0;
+    float* bn_row = (!kBnApply && p.bn_partial) ? p.bn_partial + (size_t)blockIdx.x * 2 * p.N : nullptr;
     if (bn_row) {            // this CTA's row of the batch-norm partial sums starts at zero
       for (int i = cw * 32 + lane; i < 2 * p.N; i += kConsumerThreads) bn_row[i] = 0.f;
       __threadfence_block();
@@ -330,7 +383,7 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
         ok[h] = pw < p.GW && ph < p.GH && pn < p.NB;
         o_pix[h] = p.o_off + pn * p.o_sn + ph * p.o_sh + pw * p.o_sw;
       }
-      if (p.tma_store) {
+      if (kBnApply || p.tma_store) {
         // ---- stage 64-channel slabs in smem (128B-swizzled rows) and TMA-store them ----
 #pragma unroll
         for (int s = 0; s < kBN64; ++s) {
@@ -339,8 +392,21 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
           const uint32_t slab = out_base + (uint32_t)(slab_ctr & 1) * kSlabBytes;
           if (issuer) tma_store_wait_read<1>();                    // the store that last used this slab is done reading
           named_bar_sync(1, kConsumerThreads);
-          if (s == 0) stage_slab<0>(acc, slab, row, ok[0], ok[1], lane);
-          else stage_slab<(kBN64 > 1 ? 1 : 0)>(acc, slab, row, ok[0], ok[1], lane);
+          if constexpr (kBnApply) {
+            if (ep.residual) {     // same box and swizzle as the store; rows outside the grid arrive as zeros
+              if (issuer) {
+                mbar_arrive_expect_tx(res_bar, kSlabBytes);
+                tma_load_4d(slab, rmap, res_bar, co0, tw * p.bw, th * p.bh, tn * p.bn);
+              }
+              mbar_wait(res_bar, res_phase);
+              res_phase ^= 1u;
+            }
+            if (s == 0) stage_slab_bn<0>(acc, slab, row, ok[0], ok[1], lane, ep, co0, p.N);
+            else stage_slab_bn<(kBN64 > 1 ? 1 : 0)>(acc, slab, row, ok[0], ok[1], lane, ep, co0, p.N);
+          } else {
+            if (s == 0) stage_slab<0>(acc, slab, row, ok[0], ok[1], lane);
+            else stage_slab<(kBN64 > 1 ? 1 : 0)>(acc, slab, row, ok[0], ok[1], lane);
+          }
           fence_proxy_async_smem();
           named_bar_sync(1, kConsumerThreads);
           if (issuer) {
@@ -373,6 +439,23 @@ k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUt
     if (p.tma_store && issuer) tma_store_wait_all();   // smem must outlive the bulk stores
   }
   if (CL > 1) cluster_sync_all();                         // no CTA exits while its peer may still signal it
+}
+
+template <int BN, int STAGES, int CL>
+__global__ void __launch_bounds__(kThreads, 1)
+k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
+               const __grid_constant__ CUtensorMap omap, const IgemmParams p) {
+  kmajor_body<BN, STAGES, CL, false>(amaps, bmap, omap, p, nullptr, BnEpilogue{});
+}
+
+// fprop with the inference batch norm in the epilogue (rmap: the residual, same layout as the output; unused
+// without ep.residual).  Requires p.tma_store.
+template <int BN, int STAGES, int CL>
+__global__ void __launch_bounds__(kThreads, 1)
+k_igemm_kmajor_bn(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
+                  const __grid_constant__ CUtensorMap omap, const IgemmParams p,
+                  const __grid_constant__ CUtensorMap rmap, const BnEpilogue ep) {
+  kmajor_body<BN, STAGES, CL, true>(amaps, bmap, omap, p, &rmap, ep);
 }
 
 // ----------------------------------------------------------------------------
@@ -766,11 +849,27 @@ static int launch_clustered(Kern kern, int grid, size_t smem, cudaStream_t s, Ar
   return RIGL_OK;
 }
 
+// ep != null: the batch-norm epilogue variant (k_igemm_kmajor_bn) with the residual map *rmap.
 template <int BN, int STAGES, int CL>
 static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap, const IgemmParams& p,
-                         cudaStream_t s) {
+                         cudaStream_t s, const CUtensorMap* rmap, const BnEpilogue* ep) {
+  // (the 256 bytes past the slabs hold the 2 * STAGES ring barriers and the residual barrier)
   constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 2 * (kBM * 64 * 2) + 1024 + 256;
   static_assert(smem <= 227 * 1024, "K-major kernel exceeds the shared memory of an SM");
+  static_assert(8 * (2 * STAGES + 1) <= 256, "K-major kernel barriers exceed their shared memory");
+  if (ep != nullptr) {
+    static bool configured_bn = false;
+    if (!configured_bn) {
+      RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_bn<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
+      configured_bn = true;
+    }
+    const int rc = launch_clustered<CL>(k_igemm_kmajor_bn<BN, STAGES, CL>, kmajor_grid(p), smem, s, amaps, bmap, omap,
+                                        p, *rmap, *ep);
+    if (rc != RIGL_OK) return rc;
+    RIGL_LAUNCH_CHECK("k_igemm_kmajor_bn");
+    return RIGL_OK;
+  }
   static bool configured = false;
   if (!configured) {
     RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -783,11 +882,15 @@ static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUt
 }
 
 static int dispatch_kmajor(int n_out, const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
-                           IgemmParams& p, int bn_tile, cudaStream_t s) {
+                           IgemmParams& p, int bn_tile, cudaStream_t s, const CUtensorMap* rmap = nullptr,
+                           const BnEpilogue* ep = nullptr) {
   p.n_tiles = (n_out + bn_tile - 1) / bn_tile;
   const bool mc = kmajor_use_mc(p);                        // bmap was built with kmajor_b_rows(p, bn_tile) rows
-  if (bn_tile == 64) return mc ? launch_kmajor<64, 7, 2>(amaps, bmap, omap, p, s) : launch_kmajor<64, 7, 1>(amaps, bmap, omap, p, s);
-  return mc ? launch_kmajor<128, 5, 2>(amaps, bmap, omap, p, s) : launch_kmajor<128, 5, 1>(amaps, bmap, omap, p, s);
+  if (bn_tile == 64)
+    return mc ? launch_kmajor<64, 7, 2>(amaps, bmap, omap, p, s, rmap, ep)
+              : launch_kmajor<64, 7, 1>(amaps, bmap, omap, p, s, rmap, ep);
+  return mc ? launch_kmajor<128, 5, 2>(amaps, bmap, omap, p, s, rmap, ep)
+            : launch_kmajor<128, 5, 1>(amaps, bmap, omap, p, s, rmap, ep);
 }
 
 static int pick_bn(int n_out) {
@@ -799,7 +902,7 @@ static int pick_bn(int n_out) {
 void tc_set_bn_stats_always(bool on) { g_bn_stats_always = on; }
 
 int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32, const float* bias,
-             void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial, int* bn_rows) {
+             void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial, int* bn_rows, const BnApplyArgs* bn_apply) {
   (void)ws; (void)ws_bytes;
   int rc = ensure_driver();
   if (rc != RIGL_OK) return rc;
@@ -808,6 +911,10 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
   {
     HaloParams hp = {};
     if (y != nullptr && y_f32 == nullptr && bias == nullptr && halo_fprop_ok(g, &hp)) {
+      if (bn_apply != nullptr) {          // no batch-norm epilogue on the halo kernels: plain call + rigl_bn_apply
+        set_error("fused BN apply: layer runs on the halo kernels");
+        return RIGL_ERR_UNSUPPORTED;
+      }
       if (bn_partial != nullptr) {        // the halo kernels have no statistics epilogue: the caller runs the plain
         set_error("fused BN statistics: layer runs on the halo kernels");   // call + the stats pass instead
         return RIGL_ERR_UNSUPPORTED;
@@ -860,6 +967,19 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
     p.bn_partial = bn_partial;
     p.n_tiles = (g.cout + bn_tile - 1) / bn_tile;
     if (bn_rows) *bn_rows = kmajor_grid(p);
+  }
+  if (bn_apply) {
+    if (!p.tma_store) {
+      set_error("fused BN apply needs the bf16 TMA-store epilogue");
+      return RIGL_ERR_UNSUPPORTED;
+    }
+    CUtensorMap rmap = omap;
+    if (bn_apply->residual) {            // the residual through the output's view: same boxes, same swizzle
+      rc = make_act_map(&rmap, bn_apply->residual, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
+      if (rc != RIGL_OK) return rc;
+    }
+    const BnEpilogue ep = {bn_apply->scale, bn_apply->shift, bn_apply->relu ? 1 : 0, bn_apply->residual ? 1 : 0};
+    return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s, &rmap, &ep);
   }
   return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s);
 }

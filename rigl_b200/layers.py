@@ -31,6 +31,10 @@ import os as _os
 # slab it has just staged for the TMA store), so the BN forward needs no stats pass over the activation.
 # RIGL_FUSE_BN_STATS=0: separate stats pass.
 FUSE_BN_STATS = _os.environ.get('RIGL_FUSE_BN_STATS', '1') != '0'
+# Inference forward: the conv epilogue applies the following BN's inference form (and the residual add and ReLU)
+# before the store, so the conv output is never written and re-read (rigl_masked_conv2d_fprop_bnapply, bit-identical
+# to conv + rigl_bn_apply).  RIGL_FUSE_BN_INFER=0: conv + rigl_bn_apply.
+FUSE_BN_INFER = _os.environ.get('RIGL_FUSE_BN_INFER', '1') != '0'
 _BN_ROWS = []
 
 
@@ -114,6 +118,7 @@ def side_stream(device):
 
 
 _PACKED_AHEAD = set()     # id(layer): operands already packed by pack_all for this step
+_FROZEN = set()           # id(layer): operands packed once for a whole evaluation pass (frozen_operands)
 
 
 class PackPlan(object):
@@ -186,7 +191,27 @@ def pack_all(layers):
     _PACKED_AHEAD.add(id(l))
 
 
+class frozen_operands(object):
+  """Context in which the forward passes of `layers` use their packed operands as they are: an evaluation pass
+  packs them once (workloads.Evaluator.reset) instead of once per forward.  The pack-ahead set of the training step
+  is not touched."""
+
+  def __init__(self, layers):
+    self.ids = set(id(l) for l in layers)
+
+  def __enter__(self):
+    self.added = self.ids - _FROZEN
+    _FROZEN.update(self.added)
+    return self
+
+  def __exit__(self, *exc):
+    _FROZEN.difference_update(self.added)
+    return False
+
+
 def _pack_for_forward(layer):
+  if id(layer) in _FROZEN:
+    return
   if id(layer) in _PACKED_AHEAD:
     _PACKED_AHEAD.discard(id(layer))
     return
@@ -485,13 +510,50 @@ class SparseConv2d(_MaskedLayer):
         d, src.data_ptr(), dy.data_ptr(), out.data_ptr(), 1.0 if accumulate else 0.0, ws.data_ptr(),
         ws.numel(), _cabi.stream_ptr()), 'rigl_conv2d_wgrad_dense')
 
-  def forward(self, x):
+  def bn_fusable(self, bn):
+    """Whether forward(x, bn) applies `bn` in the conv epilogue: this layer in eval mode, `bn` in its inference
+    form (eval mode, no batch statistics), autograd not recording, and FUSE_BN_INFER on."""
+    return bool(FUSE_BN_INFER and not self.training and bn.uses_inference_form() and not torch.is_grad_enabled())
+
+  def _fprop_bn(self, x, bn, residual):
+    """conv + `bn`'s inference form (+ residual, ReLU) in one launch; None where the layer's kernel has no such
+    epilogue (RIGL_ERR_UNSUPPORTED: the patch-matrix and halo layers, RIGL_FORCE_SIMT, RIGL_TMA_STORE=0)."""
+    if self.patch_mode:
+      return None
+    n, c, h, w = x.shape
+    d = self._desc(n, h, w)
+    scale, shift = bn.inference_coefficients()
+    out = torch.empty((n, self._cout, d.out_h, d.out_w), dtype=torch.bfloat16, device=x.device,
+                      memory_format=torch.channels_last)
+    if residual is not None and residual.shape != out.shape:
+      raise ValueError('residual of shape %s for an output of shape %s' % (tuple(residual.shape), tuple(out.shape)))
+    ws = _workspace(x.device, _cabi.lib().rigl_conv_workspace_bytes(d))
+    rc = _cabi.lib().rigl_masked_conv2d_fprop_bnapply(
+        d, x.data_ptr(), self.packed.data_ptr(), None if residual is None else residual.data_ptr(), scale.data_ptr(),
+        shift.data_ptr(), int(bn.relu), out.data_ptr(), ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
+    if rc == -4:          # RIGL_ERR_UNSUPPORTED (nothing launched)
+      return None
+    _cabi.check(rc, 'rigl_masked_conv2d_fprop_bnapply')
+    return out
+
+  def forward(self, x, bn=None, residual=None):
+    """conv(x), or with `bn` (a FusedBatchNormReLU over this layer's output) bn(conv(x), residual): in the
+    inference form (bn_fusable) in the conv epilogue where the layer's kernel has one, else conv + the BN module."""
     if x.dim() != 4:
       raise ValueError('Rank not supported {}'.format(x.dim()))
     if x.shape[1] != self._cin:
       raise ValueError('expected %d input channels, got %d' % (self._cin, x.shape[1]))
     x = self._as_activation(x, self._cin)
-    return _MaskedConvFn.apply(x, self.weight, None, self, False)
+    if bn is not None and self.bn_fusable(bn):
+      if residual is not None:
+        residual = residual.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+      _pack_for_forward(self)
+      out = _timed('fprop', self, lambda: self._fprop_bn(x, bn, residual))
+      if out is None:
+        out = bn(_timed('fprop', self, lambda: self._fprop(x, None, False)), residual=residual)
+      return out
+    y = _MaskedConvFn.apply(x, self.weight, None, self, False)
+    return y if bn is None else bn(y, residual=residual, producer=self)
 
 
 class SparseLinear(_MaskedLayer):

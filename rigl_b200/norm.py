@@ -31,17 +31,20 @@ class _BNFn(torch.autograd.Function):
     # written by the apply pass.  Without a ReLU (MobileNet-v2's linear bottleneck) the backward needs nothing of it.
     bits = torch.empty(rows * c // 8, dtype=torch.uint8, device=dev) if (residual is not None and mod.relu) else None
 
+    # batch statistics outside training (evaluation): the running statistics are not updated (NULL pointers)
+    rmean, rvar = (mod.running_mean, mod.running_var) if mod.training else (None, None)
+
     def run():
       if partial is not None:       # statistics already reduced by the producing conv's epilogue
         _cabi.check(_cabi.lib().rigl_bn_forward_train_partials(
             y.data_ptr(), _p(residual), gamma.data_ptr(), beta.data_ptr(), partial[0].data_ptr(), partial[1],
-            rows, c, mod.eps, mod.momentum, int(mod.relu), mod.running_mean.data_ptr(),
-            mod.running_var.data_ptr(), save[0].data_ptr(), save[1].data_ptr(), save[2].data_ptr(),
+            rows, c, mod.eps, mod.momentum, int(mod.relu), _p(rmean),
+            _p(rvar), save[0].data_ptr(), save[1].data_ptr(), save[2].data_ptr(),
             save[3].data_ptr(), out.data_ptr(), _p(bits), _cabi.stream_ptr()), 'rigl_bn_forward_train_partials')
         return
       _cabi.check(_cabi.lib().rigl_bn_forward_train(
           y.data_ptr(), _p(residual), gamma.data_ptr(), beta.data_ptr(), rows, c, mod.eps, mod.momentum,
-          int(mod.relu), mod.running_mean.data_ptr(), mod.running_var.data_ptr(), save[0].data_ptr(),
+          int(mod.relu), _p(rmean), _p(rvar), save[0].data_ptr(),
           save[1].data_ptr(), save[2].data_ptr(), save[3].data_ptr(), out.data_ptr(), ws.data_ptr(),
           ws.numel(), _p(bits), _cabi.stream_ptr()), 'rigl_bn_forward_train')
     _timed('bn_fwd', mod, run)
@@ -116,15 +119,36 @@ class FusedBatchNormReLU(nn.Module):
     self.bias = nn.Parameter(torch.zeros(channels, device=device))
     self.register_buffer('running_mean', torch.zeros(channels, device=device))
     self.register_buffer('running_var', torch.ones(channels, device=device))
+    # Evaluation with batch statistics (the reference's --use_batch_statistics): in eval mode the training-form
+    # forward runs, without updating the running statistics.
+    self.batch_statistics = False
+    self.frozen_coefficients = None     # (scale, shift) precomputed for an evaluation pass (workloads.Evaluator)
 
-  def forward(self, y, residual=None, producer=None, fork=False):
+  def inference_coefficients(self):
+    """(scale, shift) fp32 [C] of the inference form out = y * scale + shift: scale = gamma * rsqrt(var + eps),
+    shift = beta - mean * scale.  The unfused eval forward and the conv-epilogue form (SparseConv2d.forward with
+    `bn`) both take them from here, so both apply the same bits."""
+    if self.frozen_coefficients is not None:
+      return self.frozen_coefficients
+    scale = self.weight.detach() * torch.rsqrt(self.running_var + self.eps)
+    shift = self.bias.detach() - self.running_mean * scale
+    return scale, shift
+
+  def uses_inference_form(self):
+    return not self.training and not self.batch_statistics
+
+  def forward(self, y, residual=None, producer=None, fork=False, applied=False):
     """`producer`: the SparseConv2d whose output `y` is; if its epilogue emitted the batch statistics
     of exactly this tensor (layer.bn_partial), the stats pass is skipped.
     `fork`: return the activation TWICE (same storage) for its two consumers; their gradients are
     then summed inside the backward kernel instead of by a separate elementwise add (residual form, and
-    the plain form without ReLU)."""
+    the plain form without ReLU).
+    `applied`: `y` is already this module's output (the producing conv applied the inference form in its
+    epilogue); it is passed through."""
     if y.dim() != 4 or y.shape[1] != self.channels:
       raise ValueError('expected [N,%d,H,W]' % self.channels)
+    if applied:
+      return (y, y) if fork else y
     partial = None
     if producer is not None and getattr(producer, 'bn_partial', None) is not None:
       part, nrows, ptr = producer.bn_partial
@@ -138,8 +162,11 @@ class FusedBatchNormReLU(nn.Module):
       residual = residual.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
     if self.training:
       return _BNFn.apply(y, self.weight, self.bias, residual, self, partial, fork)
-    scale = self.weight.detach() * torch.rsqrt(self.running_var + self.eps)
-    shift = self.bias.detach() - self.running_mean * scale
+    if self.batch_statistics:
+      with torch.no_grad():
+        out = _BNFn.apply(y, self.weight, self.bias, residual, self, partial, False)
+      return (out, out) if fork else out
+    scale, shift = self.inference_coefficients()
     out = torch.empty_like(y, memory_format=torch.channels_last)
     n, c, h, w = y.shape
     _cabi.check(_cabi.lib().rigl_bn_apply(y.data_ptr(), _p(residual), scale.data_ptr(), shift.data_ptr(),

@@ -42,6 +42,17 @@ def _BNReLU(channels, relu=True, init_zero=False, device='cuda'):
                             decay=BATCH_NORM_DECAY, device=device)
 
 
+def conv_bn(conv, bn, x, residual=None, fork=False):
+  """bn(conv(x), residual) for a SparseConv2d `conv` feeding the FusedBatchNormReLU `bn` (`fork` as
+  FusedBatchNormReLU.forward takes it).  In the inference form (conv.bn_fusable(bn): eval mode, no autograd,
+  layers.FUSE_BN_INFER) the BN, residual add and ReLU run in the conv's epilogue where its kernel has one; otherwise
+  -- training included -- exactly the launches of bn(conv(x), producer=conv), whose epilogue may emit the BN
+  statistics.  Both modules are called, so their forward hooks fire."""
+  if conv.bn_fusable(bn):
+    return bn(conv(x, bn=bn, residual=residual), applied=True, fork=fork)
+  return bn(conv(x), residual=residual, producer=conv, fork=fork)
+
+
 # Block outputs are handed to their two consumers as two handles so that the gradient sum happens
 # inside the BN backward kernel (rigl_bn_backward) rather than in a separate elementwise add.
 FORK_BLOCK_OUTPUTS = True
@@ -74,10 +85,10 @@ class _Bottleneck(nn.Module):
     # every conv feeds a BN: its epilogue emits that BN's batch statistics (producer=...)
     if x_skip is None:
       x_skip = x
-    shortcut = x_skip if self.proj is None else self.proj_bn(self.proj(x_skip), producer=self.proj)
-    y = self.bn1(self.conv1(x), producer=self.conv1)
-    y = self.bn2(self.conv2(y), producer=self.conv2)
-    return self.bn3(self.conv3(y), residual=shortcut, producer=self.conv3, fork=fork)   # relu(BN(conv3) + shortcut)
+    shortcut = x_skip if self.proj is None else conv_bn(self.proj, self.proj_bn, x_skip)
+    y = conv_bn(self.conv1, self.bn1, x)
+    y = conv_bn(self.conv2, self.bn2, y)
+    return conv_bn(self.conv3, self.bn3, y, residual=shortcut, fork=fork)   # relu(BN(conv3) + shortcut)
 
 
 class ResNet50(nn.Module):
@@ -107,7 +118,7 @@ class ResNet50(nn.Module):
         kernel_initializer=lambda w: w.normal_(0., .01))      # resnet_model.py:713
 
   def forward(self, x):
-    x = self.initial_bn(self.initial_conv(x), producer=self.initial_conv)
+    x = conv_bn(self.initial_conv, self.initial_bn, x)
     x = max_pool_same(x, 3, 2)                      # 'SAME' 3x3/2 pool, resnet_model.py:636-642
     x_skip, last = x, len(self.blocks) - 1
     for i, blk in enumerate(self.blocks):
@@ -203,7 +214,7 @@ class MobileNetV1(nn.Module):
     x = self.initial_bn(self.initial_conv(x.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)))
     for blk in self.blocks:
       x = blk.bn_dw(blk.depthwise(x))
-      x = blk.bn_pw(blk.pointwise(x))
+      x = conv_bn(blk.pointwise, blk.bn_pw, x)
     return self.final_dense(x.mean(dim=(2, 3)))
 
 
@@ -316,13 +327,12 @@ class MobileNetV2(nn.Module):
     for i, blk in enumerate(self.blocks):
       h = x
       if blk.expand is not None:
-        h = blk.bn_expand(blk.expand(h), producer=blk.expand)
+        h = conv_bn(blk.expand, blk.bn_expand, h)
       h = blk.bn_dw(blk.depthwise(h))
       fork = FORK_BLOCK_OUTPUTS and i + 1 < len(self.blocks) and self.blocks[i + 1].shortcut
-      y = blk.bn_contraction(blk.contraction(h), residual=x_skip if blk.shortcut else None,
-                             producer=blk.contraction, fork=fork)
+      y = conv_bn(blk.contraction, blk.bn_contraction, h, residual=x_skip if blk.shortcut else None, fork=fork)
       x, x_skip = y if fork else (y, y)
-    x = self.final_bn(self.final_conv(x), producer=self.final_conv)
+    x = conv_bn(self.final_conv, self.final_bn, x)
     x = x.mean(dim=(2, 3))
     if not self.prune_last_layer:
       x = x.float()
