@@ -60,6 +60,81 @@ __host__ __device__ __forceinline__ RowGroup row_group(int C, int threads) {
 // MODE 3: (g, g*xhat), g = da [+ da2], g written to gout     (residual form without ReLU, or a plain no-ReLU BN
 //         whose output has two consumers: the linear bottleneck of MobileNet-v2).  Never touches relu_bits.
 // partial[block][2][C] fp32.
+//
+// colsum_vector: this thread's sums (s0, s1) of the 16-byte vector v (channels 8v..8v+7) over rows r0, r0 + step,
+// ... < row1.
+template <int MODE>
+__device__ __forceinline__ void colsum_vector(
+    const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ da,
+    const __nv_bfloat16* __restrict__ da2, const uint8_t* __restrict__ relu_bits, __nv_bfloat16* __restrict__ gout,
+    const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ scale,
+    const float* __restrict__ shift, int relu, long long r0, long long row1, int step, int C, int v, float (&s0)[8],
+    float (&s1)[8]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { s0[i] = 0.f; s1[i] = 0.f; }
+  float mu[8], rs[8], sc[8], sh[8];
+  if (MODE != 0) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      mu[i] = mean[8 * v + i]; rs[i] = rstd[8 * v + i];
+      sc[i] = scale[8 * v + i]; sh[i] = shift[8 * v + i];
+    }
+  }
+  // 4 rows per trip: all loads are issued before any arithmetic (memory-level parallelism)
+  for (long long rb = r0; rb < row1; rb += 4ll * step) {
+    uint4 qy[4], qd[4], qe[4];
+    uint32_t qb[4];
+    bool ok[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const long long r = rb + (long long)u * step;
+      ok[u] = r < row1;
+      if (ok[u]) {
+        const long long off = r * C + 8 * v;
+        qy[u] = *reinterpret_cast<const uint4*>(y + off);
+        if (MODE != 0) qd[u] = *reinterpret_cast<const uint4*>(da + off);
+        if (MODE == 2) qb[u] = relu_bits[off >> 3];
+        if (MODE >= 2 && da2) qe[u] = *reinterpret_cast<const uint4*>(da2 + off);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      if (!ok[u]) continue;
+      const long long off = (rb + (long long)u * step) * C + 8 * v;
+      float fy[8];
+      unpack8(qy[u], fy);
+      if (MODE == 0) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { s0[i] += fy[i]; s1[i] = fmaf(fy[i], fy[i], s1[i]); }
+      } else {
+        float g[8];
+        unpack8(qd[u], g);
+        if (MODE >= 2) {
+          if (da2) {       // the block output feeds two consumers: their gradients are summed here
+            float g2[8];   // (rounded to bf16 like the separate elementwise add it replaces)
+            unpack8(qe[u], g2);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) g[i] = __bfloat162float(__float2bfloat16(g[i] + g2[i]));
+          }
+          if (MODE == 2) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) g[i] = (!relu || ((qb[u] >> i) & 1u)) ? g[i] : 0.f;
+          }
+          *reinterpret_cast<uint4*>(gout + off) = pack8(g);
+        } else if (relu) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) g[i] = fmaf(fy[i], sc[i], sh[i]) > 0.f ? g[i] : 0.f;
+        }
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          s0[i] += g[i];
+          s1[i] = fmaf(g[i], (fy[i] - mu[i]) * rs[i], s1[i]);
+        }
+      }
+    }
+  }
+}
+
 template <int MODE, int THREADS>
 __device__ __forceinline__ void colsum_rows(
     const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ da,
@@ -72,95 +147,46 @@ __device__ __forceinline__ void colsum_rows(
   const RowGroup grp = row_group(C, THREADS);
   const int vl = grp.vl, rpi = grp.rpi;
   const int r_in = threadIdx.x / vl, v0 = threadIdx.x % vl;
-  for (int v = v0; v < V; v += vl) {            // (V > 256 only for C > 2048)
-    float s0[8], s1[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { s0[i] = 0.f; s1[i] = 0.f; }
-    float mu[8], rs[8], sc[8], sh[8];
-    if (MODE != 0) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        mu[i] = mean[8 * v + i]; rs[i] = rstd[8 * v + i];
-        sc[i] = scale[8 * v + i]; sh[i] = shift[8 * v + i];
-      }
-    }
-    if (r_in < rpi) {
-      // 4 rows per trip: all loads are issued before any arithmetic (memory-level parallelism)
-      for (long long rb = row0 + r_in; rb < row1; rb += 4ll * rpi) {
-        uint4 qy[4], qd[4], qe[4];
-        uint32_t qb[4];
-        bool ok[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const long long r = rb + (long long)u * rpi;
-          ok[u] = r < row1;
-          if (ok[u]) {
-            const long long off = r * C + 8 * v;
-            qy[u] = *reinterpret_cast<const uint4*>(y + off);
-            if (MODE != 0) qd[u] = *reinterpret_cast<const uint4*>(da + off);
-            if (MODE == 2) qb[u] = relu_bits[off >> 3];
-            if (MODE >= 2 && da2) qe[u] = *reinterpret_cast<const uint4*>(da2 + off);
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          if (!ok[u]) continue;
-          const long long off = (rb + (long long)u * rpi) * C + 8 * v;
-          float fy[8];
-          unpack8(qy[u], fy);
-          if (MODE == 0) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) { s0[i] += fy[i]; s1[i] = fmaf(fy[i], fy[i], s1[i]); }
-          } else {
-            float g[8];
-            unpack8(qd[u], g);
-            if (MODE >= 2) {
-              if (da2) {       // the block output feeds two consumers: their gradients are summed here
-                float g2[8];   // (rounded to bf16 like the separate elementwise add it replaces)
-                unpack8(qe[u], g2);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) g[i] = __bfloat162float(__float2bfloat16(g[i] + g2[i]));
-              }
-              if (MODE == 2) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) g[i] = (!relu || ((qb[u] >> i) & 1u)) ? g[i] : 0.f;
-              }
-              *reinterpret_cast<uint4*>(gout + off) = pack8(g);
-            } else if (relu) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) g[i] = fmaf(fy[i], sc[i], sh[i]) > 0.f ? g[i] : 0.f;
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              s0[i] += g[i];
-              s1[i] = fmaf(g[i], (fy[i] - mu[i]) * rs[i], s1[i]);
-            }
-          }
-        }
-      }
-    }
-    // reduce over the rpi row-threads that share this vector lane
-    if (r_in < rpi) {
-      float* dst = red + ((size_t)r_in * vl + v0) * 16;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { dst[i] = s0[i]; dst[8 + i] = s1[i]; }
-    }
-    __syncthreads();
-    if (r_in == 0) {
-      float a0[8], a1[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { a0[i] = 0.f; a1[i] = 0.f; }
-      for (int rr = 0; rr < rpi; ++rr) {
-        const float* src = red + ((size_t)rr * vl + v0) * 16;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) { a0[i] += src[i]; a1[i] += src[8 + i]; }
-      }
+  if (rpi == 1) {
+    // V > THREADS / 2: the first vl = min(V, THREADS) threads span one row; when V < THREADS the others have no
+    // vector (r_in = 1) and take no part.  Thread v0 owns vectors v0, v0 + vl, ...: their number differs between
+    // threads when vl does not divide V (V > THREADS, e.g. C = 2560 at 256 threads), so this loop has no barrier;
+    // each thread already holds the whole sums of its vectors.
+    if (r_in != 0) return;
+    for (int v = v0; v < V; v += vl) {
+      float s0[8], s1[8];
+      colsum_vector<MODE>(y, da, da2, relu_bits, gout, mean, rstd, scale, shift, relu, row0, row1, 1, C, v, s0, s1);
       float* p0 = partial_row + 8 * v;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) { p0[i] = a0[i]; p0[C + i] = a1[i]; }
+      for (int i = 0; i < 8; ++i) { p0[i] = s0[i]; p0[C + i] = s1[i]; }
     }
-    __syncthreads();
+    return;
   }
+  // V <= THREADS / 2: one vector per thread (v0), summed by rpi >= 2 row-threads whose sums are combined in shared
+  // memory (threads with r_in >= rpi, when vl does not divide THREADS, only join the barriers)
+  if (r_in < rpi) {
+    float s0[8], s1[8];
+    colsum_vector<MODE>(y, da, da2, relu_bits, gout, mean, rstd, scale, shift, relu, row0 + r_in, row1, rpi, C, v0,
+                        s0, s1);
+    float* dst = red + ((size_t)r_in * vl + v0) * 16;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { dst[i] = s0[i]; dst[8 + i] = s1[i]; }
+  }
+  __syncthreads();
+  if (r_in == 0) {
+    float a0[8], a1[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { a0[i] = 0.f; a1[i] = 0.f; }
+    for (int rr = 0; rr < rpi; ++rr) {
+      const float* src = red + ((size_t)rr * vl + v0) * 16;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { a0[i] += src[i]; a1[i] += src[8 + i]; }
+    }
+    float* p0 = partial_row + 8 * v0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { p0[i] = a0[i]; p0[C + i] = a1[i]; }
+  }
+  __syncthreads();
 }
 
 
