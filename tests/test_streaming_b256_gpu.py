@@ -43,6 +43,15 @@ def _chunks(rows, c):
   return [(a, min(a + step, rows)) for a in range(0, rows, step)]
 
 
+def _bf16_tol(want, cancelled=None):
+  """Per-element bound of _close_bf16 for the float64 values `want`."""
+  scale = float(want.abs().max()) + 1e-30
+  tol = want.abs() * 2.0 ** -7 + scale * 2.0 ** -9
+  if cancelled is not None:
+    tol = tol + cancelled * 2.0 ** -22
+  return tol
+
+
 def _close_bf16(got, want, what, cancelled=None):
   """bf16 result within 1 bf16 ulp (2^-7 relative) of the float64 value, plus 2^-9 of the chunk's largest
   magnitude for cancellation (the bound of test_bn_gpu._close_bf16, on device tensors).  `cancelled`: the summed
@@ -50,9 +59,7 @@ def _close_bf16(got, want, what, cancelled=None):
   terms, which matters where they cancel to a result near zero)."""
   got = got.double()
   scale = float(want.abs().max()) + 1e-30
-  tol = want.abs() * 2.0 ** -7 + scale * 2.0 ** -9
-  if cancelled is not None:
-    tol = tol + cancelled * 2.0 ** -22
+  tol = _bf16_tol(want, cancelled)
   err = (got - want).abs()
   bad = int((err > tol).sum())
   assert bad == 0, '%s: max err %g at scale %g (%d bad)' % (what, float(err.max()), scale, bad)
