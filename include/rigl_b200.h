@@ -274,6 +274,19 @@ RIGL_API int rigl_set_bn_stats_always(int on);
 RIGL_API int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const void* x, const void* packed,
                                               const void* residual, const float* scale, const float* shift, int relu,
                                               void* y_bf16, void* ws, size_t ws_bytes, void* stream);
+/* ReLU epilogues for convs without batch norm (VGG, vgg.py: conv2d_fixed_padding + tf.nn.relu):
+ * _fprop_relu writes y = bf16(relu(conv(x, mask*W))), equal to relu of what rigl_masked_conv2d_fprop stores (up to
+ * the sign of zero), from the K-major and halo kernels (the 3-channel first conv in patch-matrix form included).
+ * _dgrad_relu writes dx = x > 0 ? bf16(conv^T(dy, mask*W)) : 0, where x is the layer's forward input (the previous
+ * conv's ReLU output) in dx's layout and pitch: the ReLU's derivative is applied in the dgrad epilogue.  Only the
+ * single-launch stride-1 K-major dgrad has the gate.
+ * cout % 8 == 0 (dgrad: cin, cout and x_pitch too) and 16-byte aligned tensors, checked before any CUDA call.
+ * RIGL_ERR_UNSUPPORTED, with nothing launched: the CUDA-core path (RIGL_FORCE_SIMT=1), RIGL_TMA_STORE=0, and for the
+ * dgrad stride > 1 and the halo-eligible 3x3 layers; the caller then runs the plain call + rigl_relu_gate. */
+RIGL_API int rigl_masked_conv2d_fprop_relu(const rigl_conv_desc* d, const void* x, const void* packed, void* y_bf16,
+                                           void* ws, size_t ws_bytes, void* stream);
+RIGL_API int rigl_masked_conv2d_dgrad_relu(const rigl_conv_desc* d, const void* dy, const void* packed,
+                                           const void* x, void* dx, void* ws, size_t ws_bytes, void* stream);
 /* dx = conv^T(dy, mask*W). */
 RIGL_API int rigl_masked_conv2d_dgrad(const rigl_conv_desc* d, const void* dy, const void* packed,
                                       void* dx, void* ws, size_t ws_bytes, void* stream);
@@ -360,6 +373,18 @@ RIGL_API int rigl_maxpool_same_forward(const void* x, int n, int h, int w, int c
                                        void* y, uint8_t* argmax, void* stream);
 RIGL_API int rigl_maxpool_same_backward(const void* dy, const uint8_t* argmax, int n, int h, int w, int c,
                                         int ksize, int stride, void* dx, void* stream);
+/* 2x2 / stride-2 VALID max pool over a ReLU output (VGG's layers.max_pool2d([2, 2])): y [n, h/2, w/2, c] (floor).
+ * argmax: one byte per output element, the window-relative index kh*2 + kw of the first maximum in scan order, or
+ * 0xFF when that maximum is not > 0.  The backward writes every dx pixel: dy where the byte routes to it, else 0
+ * (rows / columns past the last window included), so dx is the gradient of the ReLU's input as well.
+ * h, w >= 2; c % 8 == 0; x, y, dy, dx 16-byte and argmax 8-byte aligned. */
+RIGL_API int rigl_maxpool2x2_relu_forward(const void* x, int n, int h, int w, int c, void* y, uint8_t* argmax,
+                                          void* stream);
+RIGL_API int rigl_maxpool2x2_relu_backward(const void* dy, const uint8_t* argmax, int n, int h, int w, int c,
+                                           void* dx, void* stream);
+/* out = x > 0 ? g : 0 over n bf16 elements (n % 8 == 0, 16-byte aligned); out may alias x or g.  With g == x it is
+ * the ReLU; with g a gradient it is the ReLU's backward. */
+RIGL_API int rigl_relu_gate(const void* x, const void* g, int64_t n, void* out, void* stream);
 
 /* ------------------------------------------------------------------------
  * Depthwise 3x3 convolution (stride 1 / 2, explicit padding 1), NHWC bf16, fp32 master weights [C][1][3][3]

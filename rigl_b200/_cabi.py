@@ -13,7 +13,8 @@ _lib = None
 # rigl_version() of the library these signatures and calling rules describe.  202: rigl_bn_backward takes the
 # residual form without a ReLU bitmap when relu == 0 (the linear bottleneck of MobileNet-v2).  Library version 203
 # only adds rigl_masked_conv2d_fprop_bnapply; no calling rule of an existing symbol changed, and a library without
-# the new symbol already fails its lookup in lib().
+# the new symbol already fails its lookup in lib().  204 only adds the ReLU entry points (conv epilogues, the 2x2
+# pool, rigl_relu_gate), likewise.
 ABI_VERSION = 202
 
 
@@ -89,6 +90,8 @@ SIGNATURES = {
     'rigl_masked_conv2d_fprop_bnstats': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, C.POINTER(C.c_int), _vp, _sz, _vp]),
     'rigl_masked_conv2d_fprop_bnapply': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _sz,
                                                    _vp]),
+    'rigl_masked_conv2d_fprop_relu': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _sz, _vp]),
+    'rigl_masked_conv2d_dgrad_relu': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     'rigl_masked_conv2d_dgrad': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _sz, _vp]),
     'rigl_conv2d_wgrad_dense': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _f32, _vp, _sz, _vp]),
     'rigl_im2col_nhwc': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _i64, _vp]),
@@ -114,6 +117,9 @@ SIGNATURES = {
     'rigl_depthwise3x3_wgrad': (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _f32, _vp, _sz, _vp]),
     'rigl_maxpool_same_forward': (C.c_int, [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     'rigl_maxpool_same_backward': (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
+    'rigl_maxpool2x2_relu_forward': (C.c_int, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    'rigl_maxpool2x2_relu_backward': (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    'rigl_relu_gate': (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     'rigl_set_force_simt': (C.c_int, [_i32]),
 }
 

@@ -166,6 +166,40 @@ extern "C" int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const v
   return tc_fprop(g, x, packed, y_bf16, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream, nullptr, nullptr, &bn);
 }
 
+extern "C" int rigl_masked_conv2d_fprop_relu(const rigl_conv_desc* d, const void* x, const void* packed, void* y_bf16,
+                                             void* ws, size_t ws_bytes, void* stream) {
+  ConvGeom g;
+  int rc = geom_from_desc(d, &g);
+  if (rc != RIGL_OK) return rc;
+  RIGL_REQUIRE(x && packed && y_bf16, "rigl_masked_conv2d_fprop_relu: null argument");
+  RIGL_REQUIRE(g.cout % 8 == 0, "rigl_masked_conv2d_fprop_relu: cout %d is not a multiple of 8", g.cout);
+  RIGL_REQUIRE(aligned16(x) && aligned16(y_bf16), "rigl_masked_conv2d_fprop_relu: tensors must be 16-byte aligned");
+  if (force_simt() || !tc_supported(g, 0)) {
+    set_error("rigl_masked_conv2d_fprop_relu: shape not on the tensor-core kernels");
+    return RIGL_ERR_UNSUPPORTED;
+  }
+  return tc_fprop(g, x, packed, y_bf16, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream, nullptr, nullptr,
+                  nullptr, true);
+}
+
+extern "C" int rigl_masked_conv2d_dgrad_relu(const rigl_conv_desc* d, const void* dy, const void* packed,
+                                             const void* x, void* dx, void* ws, size_t ws_bytes, void* stream) {
+  ConvGeom g;
+  int rc = geom_from_desc(d, &g);
+  if (rc != RIGL_OK) return rc;
+  RIGL_REQUIRE(dy && packed && x && dx, "rigl_masked_conv2d_dgrad_relu: null argument");
+  RIGL_REQUIRE(g.cin % 8 == 0 && g.cout % 8 == 0 && g.x_pitch % 8 == 0,
+               "rigl_masked_conv2d_dgrad_relu: cin %d, cout %d and x_pitch %d must be multiples of 8", g.cin, g.cout,
+               g.x_pitch);
+  RIGL_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dx),
+               "rigl_masked_conv2d_dgrad_relu: tensors must be 16-byte aligned");
+  if (force_simt() || !tc_supported(g, 1) || g.stride != 1) {
+    set_error("rigl_masked_conv2d_dgrad_relu: shape has no gated dgrad (stride %d)", g.stride);
+    return RIGL_ERR_UNSUPPORTED;
+  }
+  return tc_dgrad(g, dy, packed, dx, ws, ws_bytes, (cudaStream_t)stream, x);
+}
+
 extern "C" int rigl_masked_conv2d_dgrad(const rigl_conv_desc* d, const void* dy, const void* packed,
                                         void* dx, void* ws, size_t ws_bytes, void* stream) {
   ConvGeom g;

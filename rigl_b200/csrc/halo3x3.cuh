@@ -52,11 +52,11 @@ __device__ __forceinline__ void keep_frag(const uint32_t (&a)[4]) {
 // ----------------------------------------------------------------------------
 // fprop / dgrad: weights of this CTA's 64-channel N tile stay resident in shared memory.
 // grid = (CTAs over strips, N tiles).  warp 0: TMA; warpgroups 1-2: MMA + epilogue, 64 positions of each
-// 128-position M tile each.
+// 128-position M tile each.  kRelu: the fprop stores bf16(relu(D)) (stage_slab_relu).
 // ----------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads, 1)
-k_halo3x3_kmajor(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
-                 const __grid_constant__ CUtensorMap omap, const HaloParams p) {
+template <bool kRelu>
+__device__ __forceinline__ void halo_kmajor_body(const CUtensorMap& amap, const CUtensorMap& bmap,
+                                                 const CUtensorMap& omap, const HaloParams& p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t b_base = smem_base;                                   // 9 taps x 8 KB
@@ -135,7 +135,8 @@ k_halo3x3_kmajor(const __grid_constant__ CUtensorMap amap, const __grid_constant
         const uint32_t slab = out_base + (slab_ctr & 1u) * kHaloSlabBytes;
         if (issuer) tma_store_wait_read<1>();
         named_bar_sync(1, kConsumerThreads);
-        stage_slab<0>(acc, slab, row, true, true, lane);  // columns >= W and rows >= H are clipped by the store
+        if (kRelu) stage_slab_relu<0, false>(acc, slab, row, true, true, lane);
+        else stage_slab<0>(acc, slab, row, true, true, lane);   // columns >= W and rows >= H are clipped by the store
         fence_proxy_async_smem();
         named_bar_sync(1, kConsumerThreads);
         if (issuer) {
@@ -150,6 +151,18 @@ k_halo3x3_kmajor(const __grid_constant__ CUtensorMap amap, const __grid_constant
     }
     if (issuer) tma_store_wait_all();
   }
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+k_halo3x3_kmajor(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
+                 const __grid_constant__ CUtensorMap omap, const HaloParams p) {
+  halo_kmajor_body<false>(amap, bmap, omap, p);
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+k_halo3x3_kmajor_relu(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
+                      const __grid_constant__ CUtensorMap omap, const HaloParams p) {
+  halo_kmajor_body<true>(amap, bmap, omap, p);
 }
 
 // ----------------------------------------------------------------------------
@@ -319,9 +332,10 @@ static size_t halo_wgrad_ws_elems(const ConvGeom& g, const HaloParams& p) {
 }
 
 // in: activations [NB,H,W,kred] (pitch in_pitch); out: [NB,H,W,n_out] (pitch out_pitch);
-// wts: packed [tap][n_out][kpad] K-major bf16; flip = dgrad (tap (kh,kw) reads the pixel at (1-kh, 1-kw)).
+// wts: packed [tap][n_out][kpad] K-major bf16; flip = dgrad (tap (kh,kw) reads the pixel at (1-kh, 1-kw));
+// relu: k_halo3x3_kmajor_relu.
 static int halo_launch_kmajor(HaloParams p, const void* in, int kred, int in_pitch, const void* wts, int kpad,
-                              int n_out, void* out, int out_pitch, bool flip, cudaStream_t s) {
+                              int n_out, void* out, int out_pitch, bool flip, cudaStream_t s, bool relu = false) {
   for (int kh = 0; kh < 3; ++kh)
     for (int kw = 0; kw < 3; ++kw) {
       const int t = kh * 3 + kw;
@@ -342,18 +356,19 @@ static int halo_launch_kmajor(HaloParams p, const void* in, int kred, int in_pit
   rc = make_act_map(&omap, out, p.NB, p.H, p.W, n_out, out_pitch, 1, 0, 0, obox);
   if (rc != RIGL_OK) return rc;
   const size_t smem = 9 * kHaloBTapBytes + p.nbuf * (size_t)p.a_buf_bytes + 2 * kHaloSlabBytes + 1024 + 256;
-  static size_t configured = 0;
-  if (smem > configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_halo3x3_kmajor, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
+  static size_t configured[2] = {0, 0};
+  auto kern = relu ? k_halo3x3_kmajor_relu : k_halo3x3_kmajor;
+  if (smem > configured[relu]) {
+    RIGL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured[relu] = smem;
   }
   const int n_tiles = (n_out + 63) / 64;
   const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   int gx = sms / n_tiles;
   if (gx < 1) gx = 1;
   if (gx > p.total_strips) gx = p.total_strips;
-  k_halo3x3_kmajor<<<dim3((unsigned)gx, (unsigned)n_tiles), kThreads, smem, s>>>(amap, bmap, omap, p);
-  RIGL_LAUNCH_CHECK("k_halo3x3_kmajor");
+  kern<<<dim3((unsigned)gx, (unsigned)n_tiles), kThreads, smem, s>>>(amap, bmap, omap, p);
+  RIGL_LAUNCH_CHECK(relu ? "k_halo3x3_kmajor_relu" : "k_halo3x3_kmajor");
   return RIGL_OK;
 }
 

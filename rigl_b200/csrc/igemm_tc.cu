@@ -217,6 +217,37 @@ __device__ __forceinline__ void stage_slab_bn(const float (&d)[R], uint32_t slab
   }
 }
 
+// stage_slab with a ReLU (VGG, whose convs have no batch norm):
+//   fprop (kGate false): bf16(max(D, 0)), equal to relu of what stage_slab stores (rounding keeps the sign);
+//   dgrad (kGate true):  the slab already holds the layer's forward input x (TMA-loaded in the store's layout, as the
+//                        residual of stage_slab_bn); each stored value is bf16(D) where x > 0 and 0 elsewhere, the
+//                        derivative of the ReLU that produced x.  Every thread reads the words it is about to overwrite.
+template <int S, bool kGate, int R>
+__device__ __forceinline__ void stage_slab_relu(const float (&d)[R], uint32_t slab, int row, bool ok0, bool ok1,
+                                                int lane) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = row + 8 * h;
+      const int e = 4 * (8 * S + jj) + 2 * h;
+      const uint32_t dst = slab + (uint32_t)r * 128u + (uint32_t)((jj ^ (r & 7)) << 4) + (uint32_t)(lane & 3) * 4u;
+      float a = d[e], b = d[e + 1];
+      if (kGate) {
+        uint32_t xw;
+        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(xw) : "r"(dst) : "memory");
+        if (!(__uint_as_float(xw << 16) > 0.f)) a = 0.f;
+        if (!(__uint_as_float(xw & 0xffff0000u) > 0.f)) b = 0.f;
+      } else {
+        a = fmaxf(a, 0.f); b = fmaxf(b, 0.f);
+      }
+      __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+      const uint32_t w = (h ? ok1 : ok0) ? *reinterpret_cast<uint32_t*>(&v) : 0u;
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst), "r"(w) : "memory");
+    }
+  }
+}
+
 template <int R>
 __device__ __forceinline__ void zero_acc(float (&d)[R]) {
 #pragma unroll
@@ -245,11 +276,18 @@ __device__ __forceinline__ void release_stage(uint32_t bar) {
 // CL = CTAs per cluster (1 or 2).  With CL == 2 the two CTAs work on the two M tiles of a tile PAIR that share the
 // weight tile: each loads HALF of B and multicasts it into both CTAs' shared memory.  A stage is refilled only when
 // the consumers of BOTH CTAs have released it: every consumer warp arrives on the empty barrier of each CTA.
-// kBnApply: the epilogue applies the inference batch norm (stage_slab_bn) and, with ep.residual, first TMA-loads the
-// residual box at the output tile's coordinates into the staging slab (one more mbarrier, no more shared memory).
-template <int BN, int STAGES, int CL, bool kBnApply>
+// kEpi selects the epilogue at compile time:
+//   kEpiPlain     stage_slab (or direct stores), optional BN statistics;
+//   kEpiBn        the inference batch norm (stage_slab_bn); with ep.residual the residual box at the output tile's
+//                 coordinates is first TMA-loaded into the staging slab (one more mbarrier, no more shared memory);
+//   kEpiRelu      fprop with the ReLU applied (stage_slab_relu);
+//   kEpiReluGate  dgrad gated by the layer's forward input, TMA-loaded through *rmap like the residual.
+constexpr int kEpiPlain = 0, kEpiBn = 1, kEpiRelu = 2, kEpiReluGate = 3;
+template <int BN, int STAGES, int CL, int kEpi>
 __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
                                             const IgemmParams& p, const CUtensorMap* rmap, const BnEpilogue& ep) {
+  constexpr bool kBnApply = kEpi == kEpiBn;
+  constexpr bool kLoadsSlab = kEpi == kEpiBn || kEpi == kEpiReluGate;   // the residual / gate box barrier exists
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr uint32_t kABytes = kBM * kBK * 2;        // 16 KB
   constexpr uint32_t kBBytes = BN * kBK * 2;
@@ -260,7 +298,7 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
   const uint32_t bar_base = out_base + 2 * kSlabBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t res_bar = bar_base + 8u * (2 * STAGES);             // kBnApply: residual box loaded
+  const uint32_t res_bar = bar_base + 8u * (2 * STAGES);             // kLoadsSlab: residual / gate box loaded
 
   // live_cons[warpgroup][tile parity]: one liveness mask per consumer warpgroup, double-buffered over tiles
   __shared__ uint32_t live_prod[kLiveWords], live_cons[2][2][kLiveWords];
@@ -270,9 +308,9 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
     prefetch_tmap(&bmap);
     if (p.tma_store) prefetch_tmap(&omap);
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps * CL); }
-    if constexpr (kBnApply) {
+    if constexpr (kLoadsSlab) {
       mbar_init(res_bar, 1);
-      if (ep.residual) prefetch_tmap(rmap);
+      if (kEpi == kEpiReluGate || ep.residual) prefetch_tmap(rmap);
     }
     fence_barrier_init();
   }
@@ -331,7 +369,7 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
     int stage = 0; uint32_t phase = 0;
     uint32_t slab_ctr = 0;
     uint32_t res_phase = 0;
-    float* bn_row = (!kBnApply && p.bn_partial) ? p.bn_partial + (size_t)blockIdx.x * 2 * p.N : nullptr;
+    float* bn_row = (kEpi == kEpiPlain && p.bn_partial) ? p.bn_partial + (size_t)blockIdx.x * 2 * p.N : nullptr;
     if (bn_row) {            // this CTA's row of the batch-norm partial sums starts at zero
       for (int i = cw * 32 + lane; i < 2 * p.N; i += kConsumerThreads) bn_row[i] = 0.f;
       __threadfence_block();
@@ -383,7 +421,7 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
         ok[h] = pw < p.GW && ph < p.GH && pn < p.NB;
         o_pix[h] = p.o_off + pn * p.o_sn + ph * p.o_sh + pw * p.o_sw;
       }
-      if (kBnApply || p.tma_store) {
+      if (kEpi != kEpiPlain || p.tma_store) {
         // ---- stage 64-channel slabs in smem (128B-swizzled rows) and TMA-store them ----
 #pragma unroll
         for (int s = 0; s < kBN64; ++s) {
@@ -392,8 +430,8 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
           const uint32_t slab = out_base + (uint32_t)(slab_ctr & 1) * kSlabBytes;
           if (issuer) tma_store_wait_read<1>();                    // the store that last used this slab is done reading
           named_bar_sync(1, kConsumerThreads);
-          if constexpr (kBnApply) {
-            if (ep.residual) {     // same box and swizzle as the store; rows outside the grid arrive as zeros
+          if constexpr (kLoadsSlab) {
+            if (kEpi == kEpiReluGate || ep.residual) {   // same box and swizzle as the store; rows outside the grid arrive as zeros
               if (issuer) {
                 mbar_arrive_expect_tx(res_bar, kSlabBytes);
                 tma_load_4d(slab, rmap, res_bar, co0, tw * p.bw, th * p.bh, tn * p.bn);
@@ -401,8 +439,14 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
               mbar_wait(res_bar, res_phase);
               res_phase ^= 1u;
             }
+          }
+          if constexpr (kBnApply) {
             if (s == 0) stage_slab_bn<0>(acc, slab, row, ok[0], ok[1], lane, ep, co0, p.N);
             else stage_slab_bn<(kBN64 > 1 ? 1 : 0)>(acc, slab, row, ok[0], ok[1], lane, ep, co0, p.N);
+          } else if constexpr (kEpi != kEpiPlain) {
+            constexpr bool kGate = kEpi == kEpiReluGate;
+            if (s == 0) stage_slab_relu<0, kGate>(acc, slab, row, ok[0], ok[1], lane);
+            else stage_slab_relu<(kBN64 > 1 ? 1 : 0), kGate>(acc, slab, row, ok[0], ok[1], lane);
           } else {
             if (s == 0) stage_slab<0>(acc, slab, row, ok[0], ok[1], lane);
             else stage_slab<(kBN64 > 1 ? 1 : 0)>(acc, slab, row, ok[0], ok[1], lane);
@@ -445,7 +489,7 @@ template <int BN, int STAGES, int CL>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
                const __grid_constant__ CUtensorMap omap, const IgemmParams p) {
-  kmajor_body<BN, STAGES, CL, false>(amaps, bmap, omap, p, nullptr, BnEpilogue{});
+  kmajor_body<BN, STAGES, CL, kEpiPlain>(amaps, bmap, omap, p, nullptr, BnEpilogue{});
 }
 
 // fprop with the inference batch norm in the epilogue (rmap: the residual, same layout as the output; unused
@@ -455,7 +499,17 @@ __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_kmajor_bn(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
                   const __grid_constant__ CUtensorMap omap, const IgemmParams p,
                   const __grid_constant__ CUtensorMap rmap, const BnEpilogue ep) {
-  kmajor_body<BN, STAGES, CL, true>(amaps, bmap, omap, p, &rmap, ep);
+  kmajor_body<BN, STAGES, CL, kEpiBn>(amaps, bmap, omap, p, &rmap, ep);
+}
+
+// fprop with the ReLU in the epilogue (kGate false; rmap unused), or the dgrad gated by the layer's forward input
+// x > 0 (kGate true; rmap: x through dx's view, same boxes and swizzle as the store).  Requires p.tma_store.
+template <int BN, int STAGES, int CL, bool kGate>
+__global__ void __launch_bounds__(kThreads, 1)
+k_igemm_kmajor_relu(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
+                    const __grid_constant__ CUtensorMap omap, const IgemmParams p,
+                    const __grid_constant__ CUtensorMap rmap) {
+  kmajor_body<BN, STAGES, CL, kGate ? kEpiReluGate : kEpiRelu>(amaps, bmap, omap, p, &rmap, BnEpilogue{});
 }
 
 // ----------------------------------------------------------------------------
@@ -849,14 +903,36 @@ static int launch_clustered(Kern kern, int grid, size_t smem, cudaStream_t s, Ar
   return RIGL_OK;
 }
 
-// ep != null: the batch-norm epilogue variant (k_igemm_kmajor_bn) with the residual map *rmap.
+// The ReLU epilogues of k_igemm_kmajor_relu (launch_kmajor's `relu`).
+enum ReluEpi { kReluNone = 0, kReluFprop = 1, kReluGateDgrad = 2 };
+
+template <int BN, int STAGES, int CL, bool kGate>
+static int launch_kmajor_relu(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
+                              const IgemmParams& p, cudaStream_t s, const CUtensorMap& rmap, size_t smem) {
+  static bool configured = false;
+  if (!configured) {
+    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_relu<BN, STAGES, CL, kGate>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured = true;
+  }
+  const int rc = launch_clustered<CL>(k_igemm_kmajor_relu<BN, STAGES, CL, kGate>, kmajor_grid(p), smem, s, amaps, bmap,
+                                      omap, p, rmap);
+  if (rc != RIGL_OK) return rc;
+  RIGL_LAUNCH_CHECK("k_igemm_kmajor_relu");
+  return RIGL_OK;
+}
+
+// ep != null: the batch-norm epilogue variant (k_igemm_kmajor_bn) with the residual map *rmap.  relu != kReluNone:
+// the ReLU variant (k_igemm_kmajor_relu), with the gate map *rmap for kReluGateDgrad.
 template <int BN, int STAGES, int CL>
 static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap, const IgemmParams& p,
-                         cudaStream_t s, const CUtensorMap* rmap, const BnEpilogue* ep) {
+                         cudaStream_t s, const CUtensorMap* rmap, const BnEpilogue* ep, int relu) {
   // (the 256 bytes past the slabs hold the 2 * STAGES ring barriers and the residual barrier)
   constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 2 * (kBM * 64 * 2) + 1024 + 256;
   static_assert(smem <= 227 * 1024, "K-major kernel exceeds the shared memory of an SM");
   static_assert(8 * (2 * STAGES + 1) <= 256, "K-major kernel barriers exceed their shared memory");
+  if (relu == kReluFprop) return launch_kmajor_relu<BN, STAGES, CL, false>(amaps, bmap, omap, p, s, omap, smem);
+  if (relu == kReluGateDgrad) return launch_kmajor_relu<BN, STAGES, CL, true>(amaps, bmap, omap, p, s, *rmap, smem);
   if (ep != nullptr) {
     static bool configured_bn = false;
     if (!configured_bn) {
@@ -883,14 +959,14 @@ static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUt
 
 static int dispatch_kmajor(int n_out, const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
                            IgemmParams& p, int bn_tile, cudaStream_t s, const CUtensorMap* rmap = nullptr,
-                           const BnEpilogue* ep = nullptr) {
+                           const BnEpilogue* ep = nullptr, int relu = kReluNone) {
   p.n_tiles = (n_out + bn_tile - 1) / bn_tile;
   const bool mc = kmajor_use_mc(p);                        // bmap was built with kmajor_b_rows(p, bn_tile) rows
   if (bn_tile == 64)
-    return mc ? launch_kmajor<64, 7, 2>(amaps, bmap, omap, p, s, rmap, ep)
-              : launch_kmajor<64, 7, 1>(amaps, bmap, omap, p, s, rmap, ep);
-  return mc ? launch_kmajor<128, 5, 2>(amaps, bmap, omap, p, s, rmap, ep)
-            : launch_kmajor<128, 5, 1>(amaps, bmap, omap, p, s, rmap, ep);
+    return mc ? launch_kmajor<64, 7, 2>(amaps, bmap, omap, p, s, rmap, ep, relu)
+              : launch_kmajor<64, 7, 1>(amaps, bmap, omap, p, s, rmap, ep, relu);
+  return mc ? launch_kmajor<128, 5, 2>(amaps, bmap, omap, p, s, rmap, ep, relu)
+            : launch_kmajor<128, 5, 1>(amaps, bmap, omap, p, s, rmap, ep, relu);
 }
 
 static int pick_bn(int n_out) {
@@ -902,15 +978,23 @@ static int pick_bn(int n_out) {
 void tc_set_bn_stats_always(bool on) { g_bn_stats_always = on; }
 
 int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32, const float* bias,
-             void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial, int* bn_rows, const BnApplyArgs* bn_apply) {
+             void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial, int* bn_rows, const BnApplyArgs* bn_apply,
+             bool relu) {
   (void)ws; (void)ws_bytes;
   int rc = ensure_driver();
   if (rc != RIGL_OK) return rc;
   const PackedLayout L = packed_layout(g.taps(), g.cin, g.cout);
   const uint8_t* pk = static_cast<const uint8_t*>(packed);
+  if (relu && !g_tma_store) {            // both ReLU epilogues stage the output slab for the TMA store
+    set_error("fused ReLU: needs the bf16 TMA-store epilogue");
+    return RIGL_ERR_UNSUPPORTED;
+  }
   {
     HaloParams hp = {};
     if (y != nullptr && y_f32 == nullptr && bias == nullptr && halo_fprop_ok(g, &hp)) {
+      if (relu)
+        return halo_launch_kmajor(hp, x, g.cin, g.x_pitch, pk + L.off_fprop, L.cin_pad, g.cout, y, g.cout, false, s,
+                                  true);
       if (bn_apply != nullptr) {          // no batch-norm epilogue on the halo kernels: plain call + rigl_bn_apply
         set_error("fused BN apply: layer runs on the halo kernels");
         return RIGL_ERR_UNSUPPORTED;
@@ -981,11 +1065,12 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
     const BnEpilogue ep = {bn_apply->scale, bn_apply->shift, bn_apply->relu ? 1 : 0, bn_apply->residual ? 1 : 0};
     return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s, &rmap, &ep);
   }
+  if (relu) return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s, nullptr, nullptr, kReluFprop);
   return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s);
 }
 
 int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, void* ws, size_t ws_bytes,
-             cudaStream_t s) {
+             cudaStream_t s, const void* gate) {
   (void)ws; (void)ws_bytes;
   int rc = ensure_driver();
   if (rc != RIGL_OK) return rc;
@@ -994,8 +1079,17 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
   const int st = g.stride;
   {
     HaloParams hp = {};
-    if (halo_dgrad_ok(g, &hp))
+    if (halo_dgrad_ok(g, &hp)) {
+      if (gate != nullptr) {             // no gated epilogue on the halo kernels: plain call + rigl_relu_gate
+        set_error("gated dgrad: layer runs on the halo kernels");
+        return RIGL_ERR_UNSUPPORTED;
+      }
       return halo_launch_kmajor(hp, dy, g.cout, g.cout, pk + L.off_dgrad, L.cout_pad, g.cin, dx, g.x_pitch, true, s);
+    }
+  }
+  if (gate != nullptr && (st != 1 || !g_tma_store)) {   // one launch, bf16 TMA-store epilogue
+    set_error("gated dgrad: only the single-launch stride-1 dgrad with the TMA-store epilogue has the gate");
+    return RIGL_ERR_UNSUPPORTED;
   }
   // classes of input pixels by parity; each class is one launch over its sub-grid
   bool need_zero = false;
@@ -1049,6 +1143,14 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
       if (p.tma_store) {                 // dx viewed through the parity sub-grid of this launch
         rc = make_act_map(&omap, dx, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
         if (rc != RIGL_OK) return rc;
+      }
+      if (gate != nullptr) {            // x through dx's view: the gate box is the output box
+        CUtensorMap xmap;
+        rc = make_act_map(&xmap, gate, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
+        if (rc != RIGL_OK) return rc;
+        rc = dispatch_kmajor(g.cin, amaps, bmap, omap, p, bn_tile, s, &xmap, nullptr, kReluGateDgrad);
+        if (rc != RIGL_OK) return rc;
+        continue;
       }
       rc = dispatch_kmajor(g.cin, amaps, bmap, omap, p, bn_tile, s);
       if (rc != RIGL_OK) return rc;

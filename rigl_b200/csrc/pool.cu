@@ -5,6 +5,7 @@
 // Forward stores the window-relative argmax (first maximum in (kh,kw) scan order) as one byte
 // per output element; backward is a deterministic gather over the <= ceil(k/s)^2 windows that
 // cover an input pixel.  One thread = 8 channels (16-byte vectors), channels innermost.
+// Also VGG's 2x2 / stride-2 VALID pool with the ReLU's derivative in its route bytes, and the standalone ReLU gate.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -150,6 +151,97 @@ k_maxpool_bwd_3x3s2(PoolGeom g, const __nv_bfloat16* __restrict__ dy, const uint
   }
 }
 
+// ---- VGG's 2x2 / stride-2 VALID max pool (layers.max_pool2d([2, 2]), vgg.py) over a ReLU output ----
+// Forward: one thread = one output x 8 channels; it reads the four window pixels and stores the max and a route byte:
+// the window-relative index (kh * 2 + kw) of the first maximum in scan order, or kNoRoute when that maximum is not
+// > 0.  Backward: the windows are disjoint, so one thread writes its four input pixels directly (no gather);
+// gradient goes only to a routed argmax.  A maximum that is not > 0 comes from a window the ReLU zeroed entirely, so
+// the route byte also applies the ReLU's derivative: the producing conv receives the pre-activation gradient.
+// Rows / columns past the last window (odd extents, VALID floor) get zero gradient.
+constexpr uint8_t kNoRoute = 0xFF;
+
+__global__ void __launch_bounds__(256)
+k_maxpool2x2_relu_fwd(PoolGeom g, const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
+                      uint8_t* __restrict__ idx) {
+  const int V = g.c >> 3;
+  const int ow = blockIdx.x * blockDim.y + threadIdx.y, oh = blockIdx.y, n = blockIdx.z;
+  if (ow >= g.ow) return;
+  const long long p = ((long long)n * g.oh + oh) * g.ow + ow;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) {
+    uint4 raw[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      raw[j] = *reinterpret_cast<const uint4*>(
+          x + (((long long)n * g.h + 2 * oh + (j >> 1)) * g.w + 2 * ow + (j & 1)) * g.c + 8 * v);
+    uint4 o;
+    __nv_bfloat16* ob = reinterpret_cast<__nv_bfloat16*>(&o);
+    uint32_t a[2] = {0u, 0u};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      float best = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(&raw[0])[e]);
+      uint32_t arg = 0;
+#pragma unroll
+      for (int j = 1; j < 4; ++j) {
+        const float f = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(&raw[j])[e]);
+        if (f > best) { best = f; arg = (uint32_t)j; }
+      }
+      ob[e] = __float2bfloat16_rn(best);                 // exact: best is one of the bf16 inputs
+      a[e >> 2] |= (best > 0.f ? arg : (uint32_t)kNoRoute) << (8 * (e & 3));
+    }
+    *reinterpret_cast<uint4*>(y + p * g.c + 8 * v) = o;
+    *reinterpret_cast<uint2*>(idx + p * g.c + 8 * v) = make_uint2(a[0], a[1]);
+  }
+}
+
+// grid = (quad-column tiles, quad rows, images) over ceil(h/2) x ceil(w/2) quads
+__global__ void __launch_bounds__(256)
+k_maxpool2x2_relu_bwd(PoolGeom g, const __nv_bfloat16* __restrict__ dy, const uint8_t* __restrict__ idx,
+                      __nv_bfloat16* __restrict__ dx) {
+  const int V = g.c >> 3;
+  const int qw = blockIdx.x * blockDim.y + threadIdx.y, qh = blockIdx.y, n = blockIdx.z;
+  if (2 * qw >= g.w) return;
+  const bool covered = qh < g.oh && qw < g.ow;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) {
+    uint2 a = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu);
+    uint4 d = make_uint4(0u, 0u, 0u, 0u);
+    if (covered) {
+      const long long p = (((long long)n * g.oh + qh) * g.ow + qw) * g.c + 8 * v;
+      a = *reinterpret_cast<const uint2*>(idx + p);
+      d = *reinterpret_cast<const uint4*>(dy + p);
+    }
+    const uint16_t* dv = reinterpret_cast<const uint16_t*>(&d);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int hi = 2 * qh + (j >> 1), wi = 2 * qw + (j & 1);
+      if (hi >= g.h || wi >= g.w) continue;
+      uint4 o;
+      uint16_t* ov = reinterpret_cast<uint16_t*>(&o);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const uint32_t ai = ((e < 4 ? a.x : a.y) >> (8 * (e & 3))) & 0xFFu;
+        ov[e] = ai == (uint32_t)j ? dv[e] : (uint16_t)0;
+      }
+      *reinterpret_cast<uint4*>(dx + (((long long)n * g.h + hi) * g.w + wi) * g.c + 8 * v) = o;
+    }
+  }
+}
+
+// out = x > 0 ? g : 0 over n bf16 elements (8 per thread); out may alias x or g.  With g == x it is the ReLU.
+__global__ void __launch_bounds__(256)
+k_relu_gate(const __nv_bfloat16* x, const __nv_bfloat16* gr, __nv_bfloat16* out, long long n8) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 xv = reinterpret_cast<const uint4*>(x)[i];
+    const uint4 gv = reinterpret_cast<const uint4*>(gr)[i];
+    const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(&xv);
+    const uint16_t* gb = reinterpret_cast<const uint16_t*>(&gv);
+    uint4 o;
+    uint16_t* ob = reinterpret_cast<uint16_t*>(&o);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) ob[e] = __bfloat162float(xb[e]) > 0.f ? gb[e] : (uint16_t)0;
+    reinterpret_cast<uint4*>(out)[i] = o;
+  }
+}
+
 static int pool_geom(int n, int h, int w, int c, int k, int s, PoolGeom* g) {
   RIGL_REQUIRE(n > 0 && h > 0 && w > 0 && c > 0 && c % 8 == 0 && k > 0 && s > 0 && k * k <= 255,
                "maxpool: bad geometry (channels must be a multiple of 8)");
@@ -194,5 +286,51 @@ extern "C" int rigl_maxpool_same_backward(const void* dy, const uint8_t* argmax,
   const dim3 block(8, 32), grid((unsigned)((g.w + 31) / 32), (unsigned)g.h, (unsigned)n);
   k_maxpool_bwd<<<grid, block, 0, (cudaStream_t)stream>>>(g, (const __nv_bfloat16*)dy, argmax, (__nv_bfloat16*)dx);
   RIGL_LAUNCH_CHECK("k_maxpool_bwd");
+  return RIGL_OK;
+}
+
+extern "C" int rigl_maxpool2x2_relu_forward(const void* x, int n, int h, int w, int c, void* y, uint8_t* argmax,
+                                            void* stream) {
+  RIGL_REQUIRE(x && y && argmax, "rigl_maxpool2x2_relu_forward: null tensor");
+  RIGL_REQUIRE(n > 0 && h >= 2 && w >= 2 && c > 0 && c % 8 == 0,
+               "rigl_maxpool2x2_relu_forward: bad geometry (extents >= 2, channels a multiple of 8)");
+  RIGL_REQUIRE(aligned16(x) && aligned16(y) && ((uintptr_t)argmax & 7) == 0,
+               "rigl_maxpool2x2_relu_forward: x and y must be 16-byte, argmax 8-byte aligned");
+  RIGL_REQUIRE(h / 2 <= 65535 && n <= 65535, "rigl_maxpool2x2_relu_forward: extent too large");
+  const PoolGeom g = {n, h, w, c, h / 2, w / 2, 2, 2, 0};
+  const dim3 block(8, 32), grid((unsigned)((g.ow + 31) / 32), (unsigned)g.oh, (unsigned)n);
+  k_maxpool2x2_relu_fwd<<<grid, block, 0, (cudaStream_t)stream>>>(g, (const __nv_bfloat16*)x, (__nv_bfloat16*)y,
+                                                                   argmax);
+  RIGL_LAUNCH_CHECK("k_maxpool2x2_relu_fwd");
+  return RIGL_OK;
+}
+
+extern "C" int rigl_maxpool2x2_relu_backward(const void* dy, const uint8_t* argmax, int n, int h, int w, int c,
+                                             void* dx, void* stream) {
+  RIGL_REQUIRE(dy && argmax && dx, "rigl_maxpool2x2_relu_backward: null tensor");
+  RIGL_REQUIRE(n > 0 && h >= 2 && w >= 2 && c > 0 && c % 8 == 0,
+               "rigl_maxpool2x2_relu_backward: bad geometry (extents >= 2, channels a multiple of 8)");
+  RIGL_REQUIRE(aligned16(dy) && aligned16(dx) && ((uintptr_t)argmax & 7) == 0,
+               "rigl_maxpool2x2_relu_backward: dy and dx must be 16-byte, argmax 8-byte aligned");
+  RIGL_REQUIRE((h + 1) / 2 <= 65535 && n <= 65535, "rigl_maxpool2x2_relu_backward: extent too large");
+  const PoolGeom g = {n, h, w, c, h / 2, w / 2, 2, 2, 0};
+  const int qh = (h + 1) / 2, qw = (w + 1) / 2;
+  const dim3 block(8, 32), grid((unsigned)((qw + 31) / 32), (unsigned)qh, (unsigned)n);
+  k_maxpool2x2_relu_bwd<<<grid, block, 0, (cudaStream_t)stream>>>(g, (const __nv_bfloat16*)dy, argmax,
+                                                                   (__nv_bfloat16*)dx);
+  RIGL_LAUNCH_CHECK("k_maxpool2x2_relu_bwd");
+  return RIGL_OK;
+}
+
+extern "C" int rigl_relu_gate(const void* x, const void* g, int64_t n, void* out, void* stream) {
+  RIGL_REQUIRE(x && g && out, "rigl_relu_gate: null tensor");
+  RIGL_REQUIRE(n > 0 && n % 8 == 0, "rigl_relu_gate: n = %lld is not a positive multiple of 8", (long long)n);
+  RIGL_REQUIRE(aligned16(x) && aligned16(g) && aligned16(out), "rigl_relu_gate: tensors must be 16-byte aligned");
+  const long long n8 = n / 8;
+  long long blocks = (n8 + 255) / 256;
+  if (blocks > kNumSmsHint * 16) blocks = kNumSmsHint * 16;
+  k_relu_gate<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)g,
+                                                                  (__nv_bfloat16*)out, n8);
+  RIGL_LAUNCH_CHECK("k_relu_gate");
   return RIGL_OK;
 }

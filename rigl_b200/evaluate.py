@@ -27,9 +27,12 @@ from .norm import FusedBatchNormReLU
 def regularized_kernels(model):
   """The weights that carry an l2 kernel_regularizer in the reference model files: every conv and dense kernel
   (conv2d_fixed_padding, the masked layers, tf.layers.dense) except the depthwise ones, which are built with
-  weights_regularizer=None (mobilenetv1_model.py:89, mobilenetv2_model.py:89).  Biases are not regularized."""
+  weights_regularizer=None (mobilenetv1_model.py:89, mobilenetv2_model.py:89), and modules marked
+  `l2_regularized = False` (VGG's dense fc8, a contrib layers.conv2d without weights_regularizer, vgg.py:196).  Biases
+  are not regularized."""
   from .workloads import DenseConv2d
-  return [m.weight for m in model.modules() if isinstance(m, (layers._MaskedLayer, DenseConv2d, nn.Linear))]
+  return [m.weight for m in model.modules() if isinstance(m, (layers._MaskedLayer, DenseConv2d, nn.Linear))
+          and getattr(m, 'l2_regularized', True)]
 
 
 def reg_loss(model, weight_decay):

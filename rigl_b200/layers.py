@@ -35,6 +35,10 @@ FUSE_BN_STATS = _os.environ.get('RIGL_FUSE_BN_STATS', '1') != '0'
 # before the store, so the conv output is never written and re-read (rigl_masked_conv2d_fprop_bnapply, bit-identical
 # to conv + rigl_bn_apply).  RIGL_FUSE_BN_INFER=0: conv + rigl_bn_apply.
 FUSE_BN_INFER = _os.environ.get('RIGL_FUSE_BN_INFER', '1') != '0'
+# ReLU convs without batch norm (VGG): the conv epilogue writes relu(conv(x)) (rigl_masked_conv2d_fprop_relu) and the
+# next conv's dgrad epilogue applies the ReLU's derivative (rigl_masked_conv2d_dgrad_relu), so neither the ReLU nor its
+# gate is a pass over the activation.  RIGL_FUSE_RELU=0: plain conv + the standalone gate (rigl_relu_gate) everywhere.
+FUSE_RELU = _os.environ.get('RIGL_FUSE_RELU', '1') != '0'
 _BN_ROWS = []
 
 
@@ -77,6 +81,13 @@ def _timed(kind, layer, fn):
   e.record()
   Profiler.records.append((kind, layer.scope, s, e))
   return r
+
+
+def relu_gate(x, g, out):
+  """out = x > 0 ? g : 0 (bf16, same layout; `out` may be `x` or `g`): the ReLU (g = x) or its backward."""
+  _cabi.check(_cabi.lib().rigl_relu_gate(x.data_ptr(), g.data_ptr(), x.numel(), out.data_ptr(), _cabi.stream_ptr()),
+              'rigl_relu_gate')
+  return out
 
 
 def _workspace(device, nbytes):
@@ -349,8 +360,9 @@ class SparseConv2d(_MaskedLayer):
   and mask (HWIO flattened over (kh,kw,ci) is exactly the [in,out] matrix)."""
 
   def __init__(self, in_channels, units, kernel_size, strides=1, padding='SAME', name=None,
-               kernel_initializer=None, device='cuda', registry=None):
+               kernel_initializer=None, device='cuda', registry=None, out_dtype=torch.bfloat16):
     super(SparseConv2d, self).__init__()
+    self.out_dtype = out_dtype
     k = int(kernel_size[0] if isinstance(kernel_size, (tuple, list)) else kernel_size)
     s = int(strides[0] if isinstance(strides, (tuple, list)) else strides)
     if padding not in ('SAME', 'VALID', 'FIXED'):
@@ -375,6 +387,12 @@ class SparseConv2d(_MaskedLayer):
     self._use_s2d = False
     self.collect_bn_stats = False   # set by the model when a FusedBatchNormReLU consumes this output
     self.bn_partial = None
+    # Set by models whose convs are followed by a plain ReLU (VGG).  relu_out: the layer outputs relu(conv(x)), and the
+    # gradient it receives must already be the gradient of the pre-activation: every consumer gates (a gate_dgrad conv,
+    # norm.max_pool2x2_relu or norm.relu_grad_gate).  gate_dgrad: the input is such a ReLU output; the layer's dgrad
+    # applies that ReLU's derivative (x > 0) to the gradient it returns.
+    self.relu_out = False
+    self.gate_dgrad = False
 
   def pack(self):
     if self.patch_mode:      # both stem operand forms are tiny; which one runs is decided per call
@@ -445,8 +463,8 @@ class SparseConv2d(_MaskedLayer):
   def _fprop(self, x, bias, out_f32):
     n, c, h, w = x.shape
     d = self._desc(n, h, w)
-    y = torch.empty((n, self._cout, d.out_h, d.out_w), dtype=torch.bfloat16, device=x.device,
-                    memory_format=torch.channels_last)
+    y = torch.empty((n, self._cout, d.out_h, d.out_w), dtype=torch.float32 if out_f32 else torch.bfloat16,
+                    device=x.device, memory_format=torch.channels_last)
     packed, src = self.packed, x
     self._use_s2d = bool(self.s2d_mode and _cabi.lib().rigl_stem_s2d_supported(d))
     if self._use_s2d:
@@ -461,6 +479,23 @@ class SparseConv2d(_MaskedLayer):
       self._patch_cache = src = self._patches(x)
       d, packed = self._patch_desc(src.shape[0]), self.packed_patch
     ws = _workspace(x.device, _cabi.lib().rigl_conv_workspace_bytes(d))
+    if out_f32:           # (a masked classifier in conv form, VGG's fc8): fp32 logits
+      _cabi.check(_cabi.lib().rigl_masked_conv2d_fprop(
+          d, src.data_ptr(), packed.data_ptr(), None, y.data_ptr(), None, ws.data_ptr(), ws.numel(),
+          _cabi.stream_ptr()), 'rigl_masked_conv2d_fprop')
+      return y
+    if self.relu_out:
+      if FUSE_RELU:
+        rc = _cabi.lib().rigl_masked_conv2d_fprop_relu(d, src.data_ptr(), packed.data_ptr(), y.data_ptr(),
+                                                       ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
+        if rc == 0:
+          return y
+        if rc != -4:      # RIGL_ERR_UNSUPPORTED (nothing launched): plain call + the standalone gate
+          _cabi.check(rc, 'rigl_masked_conv2d_fprop_relu')
+      _cabi.check(_cabi.lib().rigl_masked_conv2d_fprop(
+          d, src.data_ptr(), packed.data_ptr(), y.data_ptr(), None, None, ws.data_ptr(),
+          ws.numel(), _cabi.stream_ptr()), 'rigl_masked_conv2d_fprop')
+      return relu_gate(y, y, y)
     self.bn_partial = None
     if self.collect_bn_stats and self.training and FUSE_BN_STATS:
       # the epilogue also emits per-CTA column sums / sums of squares of the output (BN statistics)
@@ -486,10 +521,17 @@ class SparseConv2d(_MaskedLayer):
       super(SparseConv2d, self).pack()
     dx = torch.empty_like(x, memory_format=torch.channels_last)
     ws = _workspace(x.device, _cabi.lib().rigl_conv_workspace_bytes(d))
+    if self.gate_dgrad and FUSE_RELU:
+      rc = _cabi.lib().rigl_masked_conv2d_dgrad_relu(d, dy.data_ptr(), self.packed.data_ptr(), x.data_ptr(),
+                                                     dx.data_ptr(), ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
+      if rc == 0:
+        return dx
+      if rc != -4:        # RIGL_ERR_UNSUPPORTED (nothing launched): plain call + the standalone gate
+        _cabi.check(rc, 'rigl_masked_conv2d_dgrad_relu')
     _cabi.check(_cabi.lib().rigl_masked_conv2d_dgrad(
         d, dy.data_ptr(), self.packed.data_ptr(), dx.data_ptr(), ws.data_ptr(), ws.numel(),
         _cabi.stream_ptr()), 'rigl_masked_conv2d_dgrad')
-    return dx
+    return relu_gate(x, dx, dx) if self.gate_dgrad else dx
 
   def _wgrad(self, x, dy, out, accumulate):
     n, c, h, w = x.shape
@@ -552,7 +594,7 @@ class SparseConv2d(_MaskedLayer):
       if out is None:
         out = bn(_timed('fprop', self, lambda: self._fprop(x, None, False)), residual=residual)
       return out
-    y = _MaskedConvFn.apply(x, self.weight, None, self, False)
+    y = _MaskedConvFn.apply(x, self.weight, None, self, self.out_dtype == torch.float32)
     return y if bn is None else bn(y, residual=residual, producer=self)
 
 

@@ -10,7 +10,7 @@ import torch
 from torch import nn
 
 from . import _cabi
-from .layers import _timed, _workspace
+from .layers import _timed, _workspace, relu_gate
 
 
 def _p(t):
@@ -207,3 +207,55 @@ def max_pool_same(x, ksize=3, stride=2):
   (resnet_model.py:636-642); x is [N,C,H,W] channels_last."""
   x = x.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
   return _MaxPoolFn.apply(x, int(ksize), int(stride))
+
+
+class _MaxPool2x2ReluFn(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, x):
+    n, c, h, w = x.shape
+    y = torch.empty((n, c, h // 2, w // 2), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
+    arg = torch.empty((n, h // 2, w // 2, c), dtype=torch.uint8, device=x.device)
+    _cabi.check(_cabi.lib().rigl_maxpool2x2_relu_forward(x.data_ptr(), n, h, w, c, y.data_ptr(), arg.data_ptr(),
+                                                         _cabi.stream_ptr()), 'rigl_maxpool2x2_relu_forward')
+    ctx.save_for_backward(arg)
+    ctx.geom = (n, h, w, c)
+    return y
+
+  @staticmethod
+  def backward(ctx, dy):
+    arg, = ctx.saved_tensors
+    n, h, w, c = ctx.geom
+    dy = dy.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    dx = torch.empty((n, c, h, w), dtype=torch.bfloat16, device=dy.device, memory_format=torch.channels_last)
+    _cabi.check(_cabi.lib().rigl_maxpool2x2_relu_backward(dy.data_ptr(), arg.data_ptr(), n, h, w, c, dx.data_ptr(),
+                                                          _cabi.stream_ptr()), 'rigl_maxpool2x2_relu_backward')
+    return dx
+
+
+def max_pool2x2_relu(x):
+  """layers.max_pool2d([2, 2]) (stride 2, 'VALID') of VGG (vgg.py) over a ReLU output `x` ([N,C,H,W] channels_last
+  bf16).  Its gradient goes only to each window's first maximum and only where that maximum is > 0, so it is already
+  the gradient of the ReLU's input: the producing conv (SparseConv2d.relu_out) takes it as is."""
+  x = x.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+  return _MaxPool2x2ReluFn.apply(x)
+
+
+class _ReluGradGateFn(torch.autograd.Function):
+
+  @staticmethod
+  def forward(ctx, y):
+    ctx.save_for_backward(y)
+    return y.view_as(y)
+
+  @staticmethod
+  def backward(ctx, dy):
+    y, = ctx.saved_tensors
+    dy = dy.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    return relu_gate(y, dy, torch.empty_like(y, memory_format=torch.channels_last))
+
+
+def relu_grad_gate(y):
+  """Identity on a ReLU output `y` (SparseConv2d.relu_out) whose consumer does not gate (VGG's last conv feeds the
+  global mean); the backward applies the ReLU's derivative, dy * (y > 0), with the standalone gate."""
+  return _ReluGradGateFn.apply(y.contiguous(memory_format=torch.channels_last))

@@ -7,6 +7,7 @@ that the masked conv/linear kernels and the RigL update run on:
              BN after every conv, zero-init gamma on the last BN of a block)
   MnistFC    rigl/mnist/mnist_train_eval.py:112-160 (784-300-100-10, all masked)
   MobileNetV2 rigl/imagenet_resnet/mobilenetv2_model.py (inverted residual blocks, linear bottlenecks)
+  VGG        rigl/imagenet_resnet/vgg.py (vgg_a / vgg_16 / vgg_19: 3x3 convs + ReLU, no BN; ReLU in the conv epilogues)
 BN+ReLU(+residual) run on the fused streaming kernels of csrc/bn.cu (SURVEY 8f row 1);
 pooling / loss are stock PyTorch kernels over channels_last bf16 tensors.
 """
@@ -20,7 +21,7 @@ import torch.nn.functional as F
 from . import pruning
 from . import sparse_utils
 from .layers import SparseConv2d, SparseLinear, variance_scaling_
-from .norm import FusedBatchNormReLU, max_pool_same
+from .norm import FusedBatchNormReLU, max_pool2x2_relu, max_pool_same, relu_grad_gate
 from .sparse_optimizers import SparseRigLOptimizer
 from .sparse_optimizers_base import GlobalStep
 
@@ -228,10 +229,10 @@ def _make_divisible(v, divisor=8, min_value=None):
   return new_v
 
 
-def _trunc_variance_scaling_(t, fan_in):
-  """tf.variance_scaling_initializer() defaults: scale 1, fan_in, truncated normal (|z| <= 2 sigma, the
-  untruncated standard deviation divided by 0.8796... so the truncated one is sqrt(1 / fan_in))."""
-  std = math.sqrt(1.0 / max(fan_in, 1)) / .87962566103423978
+def _trunc_variance_scaling_(t, fan_in, scale=1.0):
+  """tf.variance_scaling_initializer(scale) with its other defaults: fan_in, truncated normal (|z| <= 2 sigma, the
+  untruncated standard deviation divided by 0.8796... so the truncated one is sqrt(scale / fan_in))."""
+  std = math.sqrt(scale / max(fan_in, 1)) / .87962566103423978
   with torch.no_grad():
     nn.init.trunc_normal_(t, 0., std, -2. * std, 2. * std)
   return t
@@ -337,6 +338,83 @@ class MobileNetV2(nn.Module):
     if not self.prune_last_layer:
       x = x.float()
     return self.final_dense(x)
+
+
+# convs per stage (vgg.py network_cfg); the stages have 64, 128, 256, 512 and 512 filters times `width`
+VGG_CONFIGS = {'vgg_a': (1, 1, 2, 2, 2), 'vgg_16': (2, 2, 3, 3, 3), 'vgg_19': (2, 2, 4, 4, 4)}
+VGG_STAGE_FILTERS = (64, 128, 256, 512, 512)
+
+
+def vgg_plan(vgg_type, width=1.0):
+  """[(scope, cin, cout, pool after)] of the masked 3x3 convs of vgg_net: scopes from tf.variable_scope(vgg_type) and
+  contrib layers.repeat (scope 'convS', then 'convS_J' per repetition); a 2x2 max pool follows stages 1-4.  Every
+  width must be a multiple of 8 (the NHWC kernels move 8 channels per 16-byte vector); ValueError names the first
+  layer that is not."""
+  if vgg_type not in VGG_CONFIGS:
+    raise ValueError('vgg_type must be one of %s, got %r' % (sorted(VGG_CONFIGS), vgg_type))
+  plan, cin = [], 3
+  for s, (reps, filters) in enumerate(zip(VGG_CONFIGS[vgg_type], VGG_STAGE_FILTERS), 1):
+    cout = int(filters * width)
+    for j in range(1, reps + 1):
+      scope = '%s/conv%d/conv%d_%d' % (vgg_type, s, s, j)
+      if cout % 8:
+        raise ValueError('VGG(%s, width=%g): %s has %d channels, not a multiple of 8' % (vgg_type, width, scope, cout))
+      plan.append((scope, cin, cout, s < 5 and j == reps))
+      cin = cout
+  return plan
+
+
+class VGG(nn.Module):
+  """vgg_net (vgg.py) as the ImageNet driver builds it (--model_architecture vgg_a / vgg_16 / vgg_19, init_method
+  'baseline'): masked 3x3 / stride-1 'SAME' convs without bias, each followed by a ReLU, the first one included;
+  variance_scaling(2.0) (fan_in, truncated normal) init; a 2x2 / stride-2 'VALID' max pool after stages 1-4; then the
+  global mean over H and W and `fc8`: with prune_last_layer a masked 1x1 conv to num_classes ([1,1,C,num_classes]
+  mask, same init, fp32 logits), otherwise a dense 1x1 conv with xavier init and a zero bias that carries no l2
+  regularizer (`l2_regularized = False`, see evaluate.regularized_kernels).
+
+  The ReLUs cost no pass over the activations: every conv writes relu(conv(x)) from its epilogue
+  (SparseConv2d.relu_out) and the ReLU's derivative is applied once per edge by the consumer -- the next conv's dgrad
+  epilogue (gate_dgrad), the pool's backward (max_pool2x2_relu) or, for the last conv, relu_grad_gate."""
+
+  def __init__(self, vgg_type, num_classes=1000, width=1.0, prune_last_layer=True, device='cuda', registry=None):
+    super(VGG, self).__init__()
+    plan = vgg_plan(vgg_type, width)            # (raises before any parameter exists)
+    self.vgg_type = vgg_type
+    self.registry = registry if registry is not None else pruning.MaskedLayerRegistry()
+    reg = self.registry
+    he_init = lambda w: _trunc_variance_scaling_(w, int(np.prod(w.shape[:-1])), scale=2.0)
+    convs, self.pool_after, prev_pool = [], [], True
+    for scope, cin, cout, pool in plan:
+      conv = SparseConv2d(cin, cout, 3, strides=1, padding='SAME', name=scope, device=device, registry=reg,
+                          kernel_initializer=he_init)
+      conv.relu_out = True
+      conv.gate_dgrad = not prev_pool          # input straight from a ReLU conv (not the image, not a pool)
+      convs.append(conv)
+      self.pool_after.append(pool)
+      prev_pool = pool
+    self.convs = nn.ModuleList(convs)
+    last = plan[-1][2]
+    self.prune_last_layer = bool(prune_last_layer)
+    if self.prune_last_layer:
+      self.fc8 = SparseConv2d(last, num_classes, 1, strides=1, padding='SAME', name=vgg_type + '/fc8', device=device,
+                              registry=reg, kernel_initializer=he_init, out_dtype=torch.float32)
+    else:             # contrib layers.conv2d 1x1: not masked, fp32, xavier, zero bias, no weight regularizer
+      self.fc8 = nn.Linear(last, num_classes, device=device)
+      with torch.no_grad():
+        nn.init.xavier_uniform_(self.fc8.weight)
+        self.fc8.bias.zero_()
+      self.fc8.l2_regularized = False
+
+  def forward(self, x):
+    x = x.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
+    for conv, pool in zip(self.convs, self.pool_after):
+      x = conv(x)
+      if pool:
+        x = max_pool2x2_relu(x)
+    x = relu_grad_gate(x).mean(dim=(2, 3), keepdim=True)
+    if self.prune_last_layer:
+      return self.fc8(x).reshape(x.shape[0], -1)
+    return self.fc8(x.reshape(x.shape[0], -1).float())
 
 
 class MnistFC(nn.Module):
