@@ -155,12 +155,13 @@ def _tc_supported(cin, cout):
   return cin % 8 == 0 and cout % 8 == 0
 
 
-def _wgrad_plan(n, oh, ow, taps, cin, cout):
+def _wgrad_plan(n, oh, ow, taps, cin, cout, pitch=None):
   """The summation structure of the dense wgrad: pixels per split (`pps`), the number of splits, and the pixel
   box order that maps pixel blocks to splits.  Tensor cores: wgrad_ws_elems -- splits = ceil(2 SMs / output
   tiles), at most one per 64-pixel block, then evened out.  CUDA cores (simt_wgrad): 2048-pixel chunks in
-  flattened (n, oh, ow) order, one fp32 atomic add each."""
-  if not _tc_supported(cin, cout):
+  flattened (n, oh, ow) order, one fp32 atomic add each.  The wgrad's tensor-core test reads the row pitch of x,
+  not cin: `pitch` is that of a padded operand (a patch matrix's [rows, kpitch]), None for x's own cin."""
+  if not _tc_supported(cin if pitch is None else pitch, cout):
     chunk = 2048
     while -(-n * oh * ow // chunk) > 65535:
       chunk *= 2
@@ -271,78 +272,104 @@ def _run_layer(name, i):
   return entry, x.detach(), dy, y.detach(), x.grad, layer.masked_weights.dense_grad, layer.weight.grad
 
 
-def _layer_case(name, i):
-  torch.cuda.reset_peak_memory_stats()
-  table = _layer_table(name)
-  entry, x, dy, y, dx, dense, masked = _run_layer(name, i)
-  batch = table['batch']
-  layer = entry['layer']
-  n, h, w, cin, cout, k, s, pad, oh, ow = _geom(entry, batch)
+def _float64_layer(layer, geom, first, xs, dys, epilogue, dgrad=True):
+  """The float64 references of a masked layer with geometry `geom` (_geom), per tap as DGEMMs over chunks of whole
+  images, on the bf16-rounded masked weights (the packed operand).  xs, dys: the NHWC input and output gradient.
+
+  For every chunk of images [a, b) it calls epilogue(a, b, yr, ya, ydrop, dxr, dxa, dxdrop): the NHWC fprop
+  reference, its |terms| and its control part, then the same three for dgrad (None with dgrad=False).  The control
+  part is the centre tap of a 3x3, else the input channel with the most surviving weights (fprop: an x channel;
+  dgrad: a dy channel).  first(a, b): bool [b - a, oh, ow], the output pixels of those images that the wgrad's
+  first split adds (_first_split).  Returns (dw, |terms| of dw, the first split's share of dw), each
+  [taps, cin, cout]."""
+  n, h, w, cin, cout, k, s, pad, oh, ow = geom
   taps = k * k
-  shape = _shape_id(entry, batch)
   mask = layer.mask.to_dense().view(taps, cin, cout).double()
   wm = (layer.weight.detach().view(taps, cin, cout) * mask).to(torch.bfloat16).double()     # the packed operand
   wa = wm.abs()
   ph = max(0, (oh - 1) * s + k - h - pad)
   pw = max(0, (ow - 1) * s + k - w - pad)
-  # controls: the centre tap of a 3x3, else the input channel with the most surviving weights (fprop: x channels;
-  # dgrad: dy channels)
   ctap = taps // 2
   ci = int(mask.sum((0, 2)).argmax())
   co = int(mask.sum((0, 1)).argmax())
-  plan = _wgrad_plan(n, oh, ow, taps, cin, cout)
-  xs, dys, ys, dxs = _nhwc(x), _nhwc(dy), _nhwc(y), _nhwc(dx)
   dw = torch.zeros((taps, cin, cout), dtype=torch.float64, device=DEV)
   dw_abs, dw_first = torch.zeros_like(dw), torch.zeros_like(dw)
-  f32_out = y.dtype == torch.float32
-  r_y = r_dx = 0.0
-  ctl_y = ctl_dx = False
   step = max(1, REF_ELEMS // max(h * w * cin, oh * ow * cout))
   for a in range(0, n, step):
     b = min(a + step, n)
     xp = torch.nn.functional.pad(xs[a:b].double(), (0, 0, pad, pw, pad, ph))
     g = dys[a:b].double()
     ga = g.abs()
-    first = _first_split(plan, a, b, oh, ow)
-    g_first = g * first[..., None] if bool(first.any()) else None
+    f = first(a, b)
+    g_first = g * f[..., None] if bool(f.any()) else None
     yr = torch.zeros((b - a, oh, ow, cout), dtype=torch.float64, device=DEV)
     ya, ydrop = torch.zeros_like(yr), torch.zeros_like(yr)
-    dxp = torch.zeros_like(xp)
-    dxa, dxdrop = torch.zeros_like(xp), torch.zeros_like(xp)
+    dxp = dxa = dxdrop = None
+    if dgrad:
+      dxp = torch.zeros_like(xp)
+      dxa, dxdrop = torch.zeros_like(xp), torch.zeros_like(xp)
     for t, kh, kw, xt in _taps(xp, k, s, oh, ow):
       xt = xt.reshape(-1, cin)
       gt = g.reshape(-1, cout)
-      sl = (slice(None), slice(kh, kh + s * (oh - 1) + 1, s), slice(kw, kw + s * (ow - 1) + 1, s))
       yt = (xt @ wm[t]).view_as(yr)
-      dxt = (gt @ wm[t].T).view(b - a, oh, ow, cin)
       yr += yt
       ya += (xt.abs() @ wa[t]).view_as(yr)
-      dxp[sl] += dxt
-      dxa[sl] += (ga.reshape(-1, cout) @ wa[t].T).view(b - a, oh, ow, cin)
       if k == 1:
         ydrop += (xt[:, ci:ci + 1] @ wm[t, ci:ci + 1]).view_as(yr)
-        dxdrop[sl] += (gt[:, co:co + 1] @ wm[t][:, co:co + 1].T).view(b - a, oh, ow, cin)
       elif t == ctap:
         ydrop += yt
-        dxdrop[sl] += dxt
-      del yt, dxt
+      del yt
+      if dgrad:
+        sl = (slice(None), slice(kh, kh + s * (oh - 1) + 1, s), slice(kw, kw + s * (ow - 1) + 1, s))
+        dxt = (gt @ wm[t].T).view(b - a, oh, ow, cin)
+        dxp[sl] += dxt
+        dxa[sl] += (ga.reshape(-1, cout) @ wa[t].T).view(b - a, oh, ow, cin)
+        if k == 1:
+          dxdrop[sl] += (gt[:, co:co + 1] @ wm[t][:, co:co + 1].T).view(b - a, oh, ow, cin)
+        elif t == ctap:
+          dxdrop[sl] += dxt
+        del dxt
       dw[t] += xt.T @ gt
       dw_abs[t] += xt.abs().T @ ga.reshape(-1, cout)
       if g_first is not None:
         dw_first[t] += xt.T @ g_first.reshape(-1, cout)
     del xp, g, ga, g_first
-    crop = (slice(None), slice(pad, pad + h), slice(pad, pad + w))
-    dxr, dxa, dxdrop = dxp[crop], dxa[crop], dxdrop[crop]
+    if dgrad:
+      crop = (slice(None), slice(pad, pad + h), slice(pad, pad + w))
+      dxp, dxa, dxdrop = dxp[crop], dxa[crop], dxdrop[crop]
+    epilogue(a, b, yr, ya, ydrop, dxp, dxa, dxdrop)
+    del yr, ya, ydrop, dxp, dxa, dxdrop
+  return dw, dw_abs, dw_first
+
+
+def _layer_case(name, i):
+  torch.cuda.reset_peak_memory_stats()
+  table = _layer_table(name)
+  entry, x, dy, y, dx, dense, masked = _run_layer(name, i)
+  batch = table['batch']
+  layer = entry['layer']
+  geom = n, h, w, cin, cout, k, s, pad, oh, ow = _geom(entry, batch)
+  taps = k * k
+  shape = _shape_id(entry, batch)
+  mask = layer.mask.to_dense().view(taps, cin, cout).double()
+  plan = _wgrad_plan(n, oh, ow, taps, cin, cout)
+  xs, dys, ys, dxs = _nhwc(x), _nhwc(dy), _nhwc(y), _nhwc(dx)
+  f32_out = y.dtype == torch.float32
+  r = dict(y=0.0, dx=0.0, ctl_y=False, ctl_dx=False)
+
+  def check(a, b, yr, ya, ydrop, dxr, dxa, dxdrop):
     if f32_out:            # the classifiers: fp32 output, a sum of taps * cin products
       tol = (taps * cin + 1) * U * ya + 1e-300
-      r_y = max(r_y, _ratio(ys[a:b], yr, tol))
-      ctl_y = ctl_y or _ratio(ys[a:b], yr - ydrop, tol) > 1
+      r['y'] = max(r['y'], _ratio(ys[a:b], yr, tol))
+      r['ctl_y'] = r['ctl_y'] or _ratio(ys[a:b], yr - ydrop, tol) > 1
     else:
-      r_y = max(r_y, _bf16_ratio(ys[a:b], yr, ya))
-      ctl_y = ctl_y or _bf16_ratio(ys[a:b], yr - ydrop, ya) > 1
-    r_dx = max(r_dx, _bf16_ratio(dxs[a:b], dxr, dxa))
-    ctl_dx = ctl_dx or _bf16_ratio(dxs[a:b], dxr - dxdrop, dxa) > 1
-    del yr, ya, ydrop, dxp, dxr, dxa, dxdrop
+      r['y'] = max(r['y'], _bf16_ratio(ys[a:b], yr, ya))
+      r['ctl_y'] = r['ctl_y'] or _bf16_ratio(ys[a:b], yr - ydrop, ya) > 1
+    r['dx'] = max(r['dx'], _bf16_ratio(dxs[a:b], dxr, dxa))
+    r['ctl_dx'] = r['ctl_dx'] or _bf16_ratio(dxs[a:b], dxr - dxdrop, dxa) > 1
+
+  dw, dw_abs, dw_first = _float64_layer(layer, geom, lambda a, b: _first_split(plan, a, b, oh, ow), xs, dys, check)
+  r_y, r_dx, ctl_y, ctl_dx = r['y'], r['dx'], r['ctl_y'], r['ctl_dx']
   kern = 'simt' if not _tc_supported(cin, cout) else 'igemm'
   _report('%s fprop (%s)' % (kern, 'fp32' if f32_out else 'bf16'), shape, r_y)
   _report('%s dgrad (bf16)' % kern, shape, r_dx)
