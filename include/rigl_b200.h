@@ -269,8 +269,8 @@ RIGL_API int rigl_set_bn_stats_always(int on);
  * and re-reading the conv output.  residual (may be NULL) is bf16 NHWC in y's layout; scale / shift are fp32
  * [cout]; cout % 8 == 0; x, y and residual 16-byte aligned (checked before any CUDA call).  Only layers on the
  * K-major tensor-core kernel with the TMA-store epilogue have the variant: halo-eligible 3x3 layers, the
- * 3-channel stem, the CUDA-core path (RIGL_FORCE_SIMT=1) and RIGL_TMA_STORE=0 return RIGL_ERR_UNSUPPORTED and
- * launch nothing; the caller then runs the plain fprop + rigl_bn_apply. */
+ * 3-channel stem and the CUDA-core path (RIGL_FORCE_SIMT=1) return RIGL_ERR_UNSUPPORTED and launch nothing; the
+ * caller then runs the plain fprop + rigl_bn_apply. */
 RIGL_API int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const void* x, const void* packed,
                                               const void* residual, const float* scale, const float* shift, int relu,
                                               void* y_bf16, void* ws, size_t ws_bytes, void* stream);
@@ -281,8 +281,8 @@ RIGL_API int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const voi
  * conv's ReLU output) in dx's layout and pitch: the ReLU's derivative is applied in the dgrad epilogue.  Only the
  * single-launch stride-1 K-major dgrad has the gate.
  * cout % 8 == 0 (dgrad: cin, cout and x_pitch too) and 16-byte aligned tensors, checked before any CUDA call.
- * RIGL_ERR_UNSUPPORTED, with nothing launched: the CUDA-core path (RIGL_FORCE_SIMT=1), RIGL_TMA_STORE=0, and for the
- * dgrad stride > 1 and the halo-eligible 3x3 layers; the caller then runs the plain call + rigl_relu_gate. */
+ * RIGL_ERR_UNSUPPORTED, with nothing launched: the CUDA-core path (RIGL_FORCE_SIMT=1), and for the dgrad stride > 1
+ * and the halo-eligible 3x3 layers; the caller then runs the plain call + rigl_relu_gate. */
 RIGL_API int rigl_masked_conv2d_fprop_relu(const rigl_conv_desc* d, const void* x, const void* packed, void* y_bf16,
                                            void* ws, size_t ws_bytes, void* stream);
 RIGL_API int rigl_masked_conv2d_dgrad_relu(const rigl_conv_desc* d, const void* dy, const void* packed,

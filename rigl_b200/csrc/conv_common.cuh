@@ -64,14 +64,14 @@ struct BnApplyArgs {
 bool tc_supported(const ConvGeom& g, int which /*0 fprop, 1 dgrad, 2 wgrad*/);
 size_t tc_workspace_bytes(const ConvGeom& g);
 // bn_apply != null: RIGL_ERR_UNSUPPORTED unless the layer runs on k_igemm_kmajor with the TMA-store epilogue.
-// relu: y = bf16(relu(conv)) from the K-major or halo epilogue (RIGL_ERR_UNSUPPORTED without the TMA store).
+// relu: y = bf16(relu(conv)) from the K-major or halo epilogue.
 int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32,
              const float* bias, void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial = nullptr,
              int* bn_rows = nullptr, const BnApplyArgs* bn_apply = nullptr, bool relu = false);
 int tc_max_ctas();
 void tc_set_bn_stats_always(bool on);
 // gate != null (bf16 in dx's layout and pitch): dx = gate > 0 ? conv^T(dy) : 0 from the K-major epilogue; the halo
-// dgrad, stride > 1 and RIGL_TMA_STORE=0 return RIGL_ERR_UNSUPPORTED before any launch.
+// dgrad and stride > 1 return RIGL_ERR_UNSUPPORTED before any launch.
 int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, void* ws,
              size_t ws_bytes, cudaStream_t s, const void* gate = nullptr);
 int tc_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float beta, void* ws,

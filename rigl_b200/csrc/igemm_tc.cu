@@ -254,18 +254,6 @@ __device__ __forceinline__ void zero_acc(float (&d)[R]) {
   for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
 
-// A consumer warp's release of a ring slot: with CL == 2 the slot of BOTH CTAs is filled by both producers (each
-// multicasts its half of the shared operand), so the release goes to the empty barrier of every CTA.
-template <int CL>
-__device__ __forceinline__ void release_stage(uint32_t bar) {
-  if (CL == 1) {
-    mbar_arrive(bar);
-  } else {
-#pragma unroll
-    for (int c = 0; c < CL; ++c) mbar_arrive_cluster(bar, (uint32_t)c);
-  }
-}
-
 // Warp roles (384 threads, one CTA per SM, persistent over tiles):
 //   warp 0       : TMA producer (converged warp, one elected lane issues)   smem ring, full/empty mbarriers
 //   warps 1-3    : idle
@@ -273,9 +261,7 @@ __device__ __forceinline__ void release_stage(uint32_t bar) {
 //                  (A from shared memory, K-major), keeps its 64 x BN fp32 accumulators in registers, then runs
 //                  the epilogue for those rows: bf16 -> swizzled smem slab -> TMA store (or direct fp32/bias
 //                  stores).  The producer keeps filling the ring for the next tile meanwhile.
-// CL = CTAs per cluster (1 or 2).  With CL == 2 the two CTAs work on the two M tiles of a tile PAIR that share the
-// weight tile: each loads HALF of B and multicasts it into both CTAs' shared memory.  A stage is refilled only when
-// the consumers of BOTH CTAs have released it: every consumer warp arrives on the empty barrier of each CTA.
+// A stage is refilled once every consumer warp has arrived on its empty barrier.
 // kEpi selects the epilogue at compile time:
 //   kEpiPlain     stage_slab (or direct stores), optional BN statistics;
 //   kEpiBn        the inference batch norm (stage_slab_bn); with ep.residual the residual box at the output tile's
@@ -283,7 +269,7 @@ __device__ __forceinline__ void release_stage(uint32_t bar) {
 //   kEpiRelu      fprop with the ReLU applied (stage_slab_relu);
 //   kEpiReluGate  dgrad gated by the layer's forward input, TMA-loaded through *rmap like the residual.
 constexpr int kEpiPlain = 0, kEpiBn = 1, kEpiRelu = 2, kEpiReluGate = 3;
-template <int BN, int STAGES, int CL, int kEpi>
+template <int BN, int STAGES, int kEpi>
 __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
                                             const IgemmParams& p, const CUtensorMap* rmap, const BnEpilogue& ep) {
   constexpr bool kBnApply = kEpi == kEpiBn;
@@ -307,31 +293,28 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
     for (int i = 0; i < 4; ++i) prefetch_tmap(&amaps.a[i]);
     prefetch_tmap(&bmap);
     if (p.tma_store) prefetch_tmap(&omap);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps * CL); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
     if constexpr (kLoadsSlab) {
       mbar_init(res_bar, 1);
       if (kEpi == kEpiReluGate || ep.residual) prefetch_tmap(rmap);
     }
     fence_barrier_init();
   }
-  if (CL > 1) cluster_sync_all(); else __syncthreads();     // peers' barriers are live before any multicast
+  __syncthreads();
 
-  // Tile schedule: a "pair" = CL consecutive M tiles x one N tile; pairs are dealt round-robin to clusters, N fastest
-  // (neighbouring clusters reuse the same activation tiles in L2).  With CL == 2 the second M tile of the last pair
-  // may lie past the grid: its loads zero-fill and its stores are clipped.
-  const uint32_t cta_rank = CL > 1 ? cluster_ctarank() : 0u;
+  // Tile schedule: tiles are dealt round-robin to CTAs, N fastest (neighbouring CTAs reuse the same activation tiles
+  // in L2).
   const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int total = (m_tiles + CL - 1) / CL * p.n_tiles;
-  const int cluster_id = blockIdx.x / CL, n_clusters = gridDim.x / CL;
+  const int total = m_tiles * p.n_tiles;
+  const int first = blockIdx.x, step = gridDim.x;
   constexpr int kBN64 = (BN + 63) / 64;
-  constexpr uint16_t kMcMask = (uint16_t)((1u << CL) - 1u);
 
   if (warp == 0) {
     // ===================== TMA producer (converged warp, one elected lane issues) =====================
     int stage = 0; uint32_t phase = 0;
-    for (int tile = cluster_id; tile < total; tile += n_clusters) {
+    for (int tile = first; tile < total; tile += step) {
       const int n_tile = tile % p.n_tiles;
-      const int m_tile = (tile / p.n_tiles) * CL + (int)cta_rank;
+      const int m_tile = tile / p.n_tiles;
       const int tw = m_tile % p.tiles_w;
       const int th = (m_tile / p.tiles_w) % p.tiles_h;
       const int tn = m_tile / (p.tiles_w * p.tiles_h);
@@ -341,18 +324,13 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
         const TapInfo tap = p.taps[t];
         for (int kb = 0; kb < p.kblks; ++kb, ++j) {
           if (masked && !((live_prod[j >> 5] >> (j & 31)) & 1u)) continue;
-          if (CL > 1) mbar_wait_cluster(empty_bar(stage), phase ^ 1u);
-          else mbar_wait(empty_bar(stage), phase ^ 1u);
+          mbar_wait(empty_bar(stage), phase ^ 1u);
           if (elect_one()) {
             const uint32_t a_dst = smem_base + stage * kStageBytes;
-            mbar_arrive_expect_tx(full_bar(stage), kStageBytes);      // my A + both halves of B
+            mbar_arrive_expect_tx(full_bar(stage), kStageBytes);      // A + B
             tma_load_4d(a_dst, &amaps.a[tap.map_id], full_bar(stage), kb * kBK, tw * p.bw + tap.dw,
                         th * p.bh + tap.dh, tn * p.bn);
-            if (CL > 1)        // my half of the weight tile, multicast to every CTA of the cluster
-              tma_load_3d_mc(a_dst + kABytes + cta_rank * (uint32_t)(BN / CL) * 128u, &bmap, full_bar(stage),
-                             kb * kBK, n_tile * BN + (int)cta_rank * (BN / CL), tap.b_tap, kMcMask);
-            else
-              tma_load_3d(a_dst + kABytes, &bmap, full_bar(stage), kb * kBK, n_tile * BN, tap.b_tap);
+            tma_load_3d(a_dst + kABytes, &bmap, full_bar(stage), kb * kBK, n_tile * BN, tap.b_tap);
           }
           __syncwarp();
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
@@ -376,9 +354,9 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
       named_bar_sync(1, kConsumerThreads);
     }
     int tile_ctr = 0;
-    for (int tile = cluster_id; tile < total; tile += n_clusters, ++tile_ctr) {
+    for (int tile = first; tile < total; tile += step, ++tile_ctr) {
       const int n_tile = tile % p.n_tiles;
-      const int m_tile = (tile / p.n_tiles) * CL + (int)cta_rank;
+      const int m_tile = tile / p.n_tiles;
       // the first warp of the warpgroup builds the tile's liveness mask, the other three wait for it
       uint32_t* live = live_cons[wg][tile_ctr & 1];
       if ((cw & 3) == 0) build_live_mask<kBN64>(p, n_tile, lane, live);
@@ -400,13 +378,13 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
           Wgmma<BN>::template ss<0, 0>(acc, da + 2 * k, db + 2 * k);
         wgmma_commit();
         wgmma_wait<1>();                                  // the previous stage's MMAs have read their operands
-        if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
       wgmma_wait<0>();
       fence_regs(acc);
-      if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
 
       const int tw = m_tile % p.tiles_w;
       const int th = (m_tile / p.tiles_w) % p.tiles_h;
@@ -482,34 +460,33 @@ __device__ __forceinline__ void kmajor_body(const TMaps4& amaps, const CUtensorM
     }
     if (p.tma_store && issuer) tma_store_wait_all();   // smem must outlive the bulk stores
   }
-  if (CL > 1) cluster_sync_all();                         // no CTA exits while its peer may still signal it
 }
 
-template <int BN, int STAGES, int CL>
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_kmajor(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
                const __grid_constant__ CUtensorMap omap, const IgemmParams p) {
-  kmajor_body<BN, STAGES, CL, kEpiPlain>(amaps, bmap, omap, p, nullptr, BnEpilogue{});
+  kmajor_body<BN, STAGES, kEpiPlain>(amaps, bmap, omap, p, nullptr, BnEpilogue{});
 }
 
 // fprop with the inference batch norm in the epilogue (rmap: the residual, same layout as the output; unused
 // without ep.residual).  Requires p.tma_store.
-template <int BN, int STAGES, int CL>
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_kmajor_bn(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
                   const __grid_constant__ CUtensorMap omap, const IgemmParams p,
                   const __grid_constant__ CUtensorMap rmap, const BnEpilogue ep) {
-  kmajor_body<BN, STAGES, CL, kEpiBn>(amaps, bmap, omap, p, &rmap, ep);
+  kmajor_body<BN, STAGES, kEpiBn>(amaps, bmap, omap, p, &rmap, ep);
 }
 
 // fprop with the ReLU in the epilogue (kGate false; rmap unused), or the dgrad gated by the layer's forward input
 // x > 0 (kGate true; rmap: x through dx's view, same boxes and swizzle as the store).  Requires p.tma_store.
-template <int BN, int STAGES, int CL, bool kGate>
+template <int BN, int STAGES, bool kGate>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_kmajor_relu(const __grid_constant__ TMaps4 amaps, const __grid_constant__ CUtensorMap bmap,
                     const __grid_constant__ CUtensorMap omap, const IgemmParams p,
                     const __grid_constant__ CUtensorMap rmap) {
-  kmajor_body<BN, STAGES, CL, kGate ? kEpiReluGate : kEpiRelu>(amaps, bmap, omap, p, &rmap, BnEpilogue{});
+  kmajor_body<BN, STAGES, kGate ? kEpiReluGate : kEpiRelu>(amaps, bmap, omap, p, &rmap, BnEpilogue{});
 }
 
 // ----------------------------------------------------------------------------
@@ -529,10 +506,8 @@ struct WgradParams {
 };
 
 // Same warp roles as k_igemm_kmajor; consumer warpgroup w owns input channels 64w..64w+63 of the unit (the
-// w-th 64-channel x box of a stage is its whole A operand).  CL = CTAs per cluster (1 or 2): the dY tile depends only
-// on (pixel block, N tile), so with CL == 2 two work units that differ in (tap, M tile) share it; each CTA fetches
-// half of the dY boxes and multicasts them to both (same protocol as k_igemm_kmajor).
-template <int BN, int STAGES, int CL>
+// w-th 64-channel x box of a stage is its whole A operand).
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUtensorMap dymap,
               const WgradParams p) {
@@ -542,8 +517,6 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
   constexpr uint32_t kStageBytes = kABytes + kBBytes;
   constexpr uint32_t kBox = 64 * 64 * 2;             // 8 KB: 64 pixels x 64 channels
   constexpr int kBBoxes = BN / 64;
-  static_assert(CL == 1 || kBBoxes % CL == 0, "multicast splits the dY boxes between the CTAs");
-  constexpr uint16_t kMcMask = (uint16_t)((1u << CL) - 1u);
 
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + STAGES * kStageBytes;
@@ -554,37 +527,34 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
   if (threadIdx.x == 0) {
     for (int i = 0; i < 4; ++i) prefetch_tmap(&xmaps.a[i]);
     prefetch_tmap(&dymap);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps * CL); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), kConsumerWarps); }
     fence_barrier_init();
   }
-  if (CL > 1) cluster_sync_all(); else __syncthreads();
+  __syncthreads();
 
-  // Work units: (split, N tile, M index) with M index = tap * m_tiles + m_tile; a cluster takes CL consecutive M
-  // indices of one (split, N tile).  Indices past the end are idle partners: their x boxes are requested out of
-  // bounds (zero fill) and nothing is stored.
-  const uint32_t cta_rank = CL > 1 ? cluster_ctarank() : 0u;
+  // Work units: (split, N tile, M index) with M index = tap * m_tiles + m_tile, dealt round-robin to CTAs.
+  // `live` (mi < mcount) always holds; the guarded selects below are kept because nvcc cannot prove it, and dropping
+  // them reschedules the main loop around the wgmma.
   const int mcount = p.ntaps * p.m_tiles;
-  const int m_groups = (mcount + CL - 1) / CL;
-  const int groups_per_split = m_groups * p.n_tiles;
-  const int total_groups = groups_per_split * p.splits;
-  const int cluster_id = blockIdx.x / CL, n_clusters = gridDim.x / CL;
+  const int units_per_split = mcount * p.n_tiles;
+  const int total_units = units_per_split * p.splits;
+  const int first = blockIdx.x, step = gridDim.x;
 
   if (warp == 0) {
     int stage = 0; uint32_t phase = 0;                     // converged warp, one elected lane issues
-    for (int q = cluster_id; q < total_groups; q += n_clusters) {
-      const int split = q / groups_per_split;
-      const int r = q % groups_per_split;
+    for (int q = first; q < total_units; q += step) {
+      const int split = q / units_per_split;
+      const int r = q % units_per_split;
       const int n_tile = r % p.n_tiles;
-      const int mi = (r / p.n_tiles) * CL + (int)cta_rank;
+      const int mi = r / p.n_tiles;
       const bool live = mi < mcount;
       const TapInfo tap = p.taps[live ? mi / p.m_tiles : 0];
-      const int c_base = live ? (mi % p.m_tiles) * kBM : (1 << 28);     // idle partner: out of bounds
+      const int c_base = live ? (mi % p.m_tiles) * kBM : (1 << 28);
       const int pb0 = split * p.pblocks_per_split;
       const int pb1 = min(pb0 + p.pblocks_per_split, p.pblocks);
       int tw = pb0 % p.tiles_w, th = (pb0 / p.tiles_w) % p.tiles_h, tn = pb0 / (p.tiles_w * p.tiles_h);
       for (int pb = pb0; pb < pb1; ++pb) {
-        if (CL > 1) mbar_wait_cluster(empty_bar(stage), phase ^ 1u);
-        else mbar_wait(empty_bar(stage), phase ^ 1u);
+        mbar_wait(empty_bar(stage), phase ^ 1u);
         if (elect_one()) {
           const uint32_t a_dst = smem_base + stage * kStageBytes;
           const uint32_t b_dst = a_dst + kABytes;
@@ -593,19 +563,10 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
           for (int h = 0; h < kBM / 64; ++h)
             tma_load_4d(a_dst + h * kBox, &xmaps.a[tap.map_id], full_bar(stage), c_base + h * 64,
                         tw * p.bw + tap.dw, th * p.bh + tap.dh, tn * p.bn);
-          if (CL > 1) {
 #pragma unroll
-            for (int hh = 0; hh < kBBoxes / CL; ++hh) {
-              const int h = (int)cta_rank * (kBBoxes / CL) + hh;
-              tma_load_4d_mc(b_dst + h * kBox, &dymap, full_bar(stage), n_tile * BN + h * 64, tw * p.bw,
-                             th * p.bh, tn * p.bn, kMcMask);
-            }
-          } else {
-#pragma unroll
-            for (int h = 0; h < kBBoxes; ++h)
-              tma_load_4d(b_dst + h * kBox, &dymap, full_bar(stage), n_tile * BN + h * 64, tw * p.bw,
-                          th * p.bh, tn * p.bn);
-          }
+          for (int h = 0; h < kBBoxes; ++h)
+            tma_load_4d(b_dst + h * kBox, &dymap, full_bar(stage), n_tile * BN + h * 64, tw * p.bw,
+                        th * p.bh, tn * p.bn);
         }
         __syncwarp();
         if (++tw == p.tiles_w) { tw = 0; if (++th == p.tiles_h) { th = 0; ++tn; } }   // next pixel block (no divisions)
@@ -618,11 +579,11 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
     const int row = 64 * wg + 16 * (cw & 3) + (lane >> 2);
     float acc[BN / 2];
     int stage = 0; uint32_t phase = 0;
-    for (int q = cluster_id; q < total_groups; q += n_clusters) {
-      const int split = q / groups_per_split;
-      const int r = q % groups_per_split;
+    for (int q = first; q < total_units; q += step) {
+      const int split = q / units_per_split;
+      const int r = q % units_per_split;
       const int n_tile = r % p.n_tiles;
-      const int mi = (r / p.n_tiles) * CL + (int)cta_rank;
+      const int mi = r / p.n_tiles;
       const bool live = mi < mcount;
       const int tap_idx = live ? mi / p.m_tiles : 0;
       const int pb0 = split * p.pblocks_per_split;
@@ -641,15 +602,15 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
           Wgmma<BN>::template ss<1, 1>(acc, da + 128 * k, db + 128 * k);
         wgmma_commit();
         wgmma_wait<1>();
-        if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1u; }
       }
       wgmma_wait<0>();
       fence_regs(acc);
-      if (prev >= 0 && lane == 0) release_stage<CL>(empty_bar(prev));
+      if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
 
-      const int m0 = live ? (mi % p.m_tiles) * kBM : p.ci;            // idle partner stores nothing
+      const int m0 = live ? (mi % p.m_tiles) * kBM : p.ci;
       float* base = p.out + (long long)split * p.split_stride + (long long)p.taps[tap_idx].b_tap * p.ci * p.co;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -665,7 +626,6 @@ k_igemm_wgrad(const __grid_constant__ TMaps4 xmaps, const __grid_constant__ CUte
       }
     }
   }
-  if (CL > 1) cluster_sync_all();                         // no CTA exits while its peer may still signal it
 }
 
 // dw = beta * dw + sum_s partial[s]   (fixed summation order => deterministic)
@@ -697,10 +657,6 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 static EncodeTiledFn g_encode = nullptr;
-static bool g_tma_store = true;     // RIGL_TMA_STORE=0 falls back to per-thread global stores
-// RIGL_CLUSTER_MC=1: 2-CTA clusters whose CTAs share the weight tile (fprop/dgrad) or the dY tile (wgrad): each loads
-// half of it and multicasts it to both, halving those L2 -> SM bytes.  Opt-in; the single-CTA kernels are the default.
-static bool g_cluster_mc = false;
 static bool g_bn_stats_always = false;   // rigl_set_bn_stats_always: epilogue statistics for every supported shape (tests)
 static bool g_halo = true;          // RIGL_HALO3X3=0: 3x3/s1 layers with <= 64 channels use the generic kernels
 static int g_num_sms = 0;
@@ -717,9 +673,7 @@ static void init_driver() {
     return;
   }
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  if (const char* e = getenv("RIGL_TMA_STORE")) g_tma_store = !(e[0] == '0');
   if (const char* e = getenv("RIGL_HALO3X3")) g_halo = !(e[0] == '0');
-  if (const char* e = getenv("RIGL_CLUSTER_MC")) g_cluster_mc = (e[0] == '1');
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
@@ -866,93 +820,56 @@ size_t tc_workspace_bytes(const ConvGeom& g) {
   return elems * sizeof(float) + 256;
 }
 
-static bool kmajor_use_mc(const IgemmParams& p) {      // multicast needs a partner M tile
-  return g_cluster_mc && p.tiles_w * p.tiles_h * p.tiles_n >= 2;
-}
-static int kmajor_b_rows(const IgemmParams& p, int bn_tile) {   // with the multicast each CTA fetches half of B
-  return kmajor_use_mc(p) ? bn_tile / 2 : bn_tile;
-}
-
 static int kmajor_grid(const IgemmParams& p) {         // CTAs the K-major launcher will use (p.n_tiles set)
-  const int cl = kmajor_use_mc(p) ? 2 : 1;
-  const int m_tiles = p.tiles_w * p.tiles_h * p.tiles_n;
-  const int pairs = ((m_tiles + cl - 1) / cl) * p.n_tiles;
-  int clusters = g_num_sms / cl;
-  if (pairs < clusters) clusters = pairs;
-  return clusters * cl;
-}
-
-// Launch with a cluster of CL CTAs along x (CL == 1: a plain launch).
-template <int CL, typename Kern, typename... Args>
-static int launch_clustered(Kern kern, int grid, size_t smem, cudaStream_t s, Args... args) {
-  if (CL == 1) {
-    kern<<<(unsigned)grid, kThreads, smem, s>>>(args...);
-    return RIGL_OK;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  RIGL_CUDA(cudaLaunchKernelEx(&cfg, kern, args...));
-  return RIGL_OK;
+  const int tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;
+  return tiles < g_num_sms ? tiles : g_num_sms;
 }
 
 // The ReLU epilogues of k_igemm_kmajor_relu (launch_kmajor's `relu`).
 enum ReluEpi { kReluNone = 0, kReluFprop = 1, kReluGateDgrad = 2 };
 
-template <int BN, int STAGES, int CL, bool kGate>
+template <int BN, int STAGES, bool kGate>
 static int launch_kmajor_relu(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
                               const IgemmParams& p, cudaStream_t s, const CUtensorMap& rmap, size_t smem) {
   static bool configured = false;
   if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_relu<BN, STAGES, CL, kGate>,
+    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_relu<BN, STAGES, kGate>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  const int rc = launch_clustered<CL>(k_igemm_kmajor_relu<BN, STAGES, CL, kGate>, kmajor_grid(p), smem, s, amaps, bmap,
-                                      omap, p, rmap);
-  if (rc != RIGL_OK) return rc;
+  k_igemm_kmajor_relu<BN, STAGES, kGate><<<kmajor_grid(p), kThreads, smem, s>>>(amaps, bmap, omap, p, rmap);
   RIGL_LAUNCH_CHECK("k_igemm_kmajor_relu");
   return RIGL_OK;
 }
 
 // ep != null: the batch-norm epilogue variant (k_igemm_kmajor_bn) with the residual map *rmap.  relu != kReluNone:
 // the ReLU variant (k_igemm_kmajor_relu), with the gate map *rmap for kReluGateDgrad.
-template <int BN, int STAGES, int CL>
+template <int BN, int STAGES>
 static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap, const IgemmParams& p,
                          cudaStream_t s, const CUtensorMap* rmap, const BnEpilogue* ep, int relu) {
   // (the 256 bytes past the slabs hold the 2 * STAGES ring barriers and the residual barrier)
   constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 2 * (kBM * 64 * 2) + 1024 + 256;
   static_assert(smem <= 227 * 1024, "K-major kernel exceeds the shared memory of an SM");
   static_assert(8 * (2 * STAGES + 1) <= 256, "K-major kernel barriers exceed their shared memory");
-  if (relu == kReluFprop) return launch_kmajor_relu<BN, STAGES, CL, false>(amaps, bmap, omap, p, s, omap, smem);
-  if (relu == kReluGateDgrad) return launch_kmajor_relu<BN, STAGES, CL, true>(amaps, bmap, omap, p, s, *rmap, smem);
+  if (relu == kReluFprop) return launch_kmajor_relu<BN, STAGES, false>(amaps, bmap, omap, p, s, omap, smem);
+  if (relu == kReluGateDgrad) return launch_kmajor_relu<BN, STAGES, true>(amaps, bmap, omap, p, s, *rmap, smem);
   if (ep != nullptr) {
     static bool configured_bn = false;
     if (!configured_bn) {
-      RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_bn<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_bn<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)smem));
       configured_bn = true;
     }
-    const int rc = launch_clustered<CL>(k_igemm_kmajor_bn<BN, STAGES, CL>, kmajor_grid(p), smem, s, amaps, bmap, omap,
-                                        p, *rmap, *ep);
-    if (rc != RIGL_OK) return rc;
+    k_igemm_kmajor_bn<BN, STAGES><<<kmajor_grid(p), kThreads, smem, s>>>(amaps, bmap, omap, p, *rmap, *ep);
     RIGL_LAUNCH_CHECK("k_igemm_kmajor_bn");
     return RIGL_OK;
   }
   static bool configured = false;
   if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  const int rc = launch_clustered<CL>(k_igemm_kmajor<BN, STAGES, CL>, kmajor_grid(p), smem, s, amaps, bmap, omap, p);
-  if (rc != RIGL_OK) return rc;
+  k_igemm_kmajor<BN, STAGES><<<kmajor_grid(p), kThreads, smem, s>>>(amaps, bmap, omap, p);
   RIGL_LAUNCH_CHECK("k_igemm_kmajor");
   return RIGL_OK;
 }
@@ -961,12 +878,8 @@ static int dispatch_kmajor(int n_out, const TMaps4& amaps, const CUtensorMap& bm
                            IgemmParams& p, int bn_tile, cudaStream_t s, const CUtensorMap* rmap = nullptr,
                            const BnEpilogue* ep = nullptr, int relu = kReluNone) {
   p.n_tiles = (n_out + bn_tile - 1) / bn_tile;
-  const bool mc = kmajor_use_mc(p);                        // bmap was built with kmajor_b_rows(p, bn_tile) rows
-  if (bn_tile == 64)
-    return mc ? launch_kmajor<64, 7, 2>(amaps, bmap, omap, p, s, rmap, ep, relu)
-              : launch_kmajor<64, 7, 1>(amaps, bmap, omap, p, s, rmap, ep, relu);
-  return mc ? launch_kmajor<128, 5, 2>(amaps, bmap, omap, p, s, rmap, ep, relu)
-            : launch_kmajor<128, 5, 1>(amaps, bmap, omap, p, s, rmap, ep, relu);
+  if (bn_tile == 64) return launch_kmajor<64, 7>(amaps, bmap, omap, p, s, rmap, ep, relu);
+  return launch_kmajor<128, 5>(amaps, bmap, omap, p, s, rmap, ep, relu);
 }
 
 static int pick_bn(int n_out) {
@@ -985,10 +898,6 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
   if (rc != RIGL_OK) return rc;
   const PackedLayout L = packed_layout(g.taps(), g.cin, g.cout);
   const uint8_t* pk = static_cast<const uint8_t*>(packed);
-  if (relu && !g_tma_store) {            // both ReLU epilogues stage the output slab for the TMA store
-    set_error("fused ReLU: needs the bf16 TMA-store epilogue");
-    return RIGL_ERR_UNSUPPORTED;
-  }
   {
     HaloParams hp = {};
     if (y != nullptr && y_f32 == nullptr && bias == nullptr && halo_fprop_ok(g, &hp)) {
@@ -1034,29 +943,21 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
   CUtensorMap bmap;
   const uint64_t bdims[3] = {(uint64_t)L.cin_pad, (uint64_t)g.cout, (uint64_t)g.taps()};
   const uint64_t bstr[2] = {(uint64_t)L.cin_pad * 2, (uint64_t)g.cout * L.cin_pad * 2};
-  const uint32_t bbox[3] = {(uint32_t)kBK, (uint32_t)kmajor_b_rows(p, bn_tile), 1};
+  const uint32_t bbox[3] = {(uint32_t)kBK, (uint32_t)bn_tile, 1};
   rc = make_tmap(&bmap, pk + L.off_fprop, 3, bdims, bstr, bbox);
   if (rc != RIGL_OK) return rc;
   CUtensorMap omap = bmap;
-  p.tma_store = (y != nullptr && y_f32 == nullptr && bias == nullptr && g_tma_store) ? 1 : 0;
+  p.tma_store = (y != nullptr && y_f32 == nullptr && bias == nullptr) ? 1 : 0;
   if (p.tma_store) {
     rc = make_act_map(&omap, y, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
     if (rc != RIGL_OK) return rc;
   }
   if (bn_partial) {
-    if (!p.tma_store) {
-      set_error("fused BN statistics need the bf16 TMA-store epilogue");
-      return RIGL_ERR_UNSUPPORTED;
-    }
     p.bn_partial = bn_partial;
     p.n_tiles = (g.cout + bn_tile - 1) / bn_tile;
     if (bn_rows) *bn_rows = kmajor_grid(p);
   }
   if (bn_apply) {
-    if (!p.tma_store) {
-      set_error("fused BN apply needs the bf16 TMA-store epilogue");
-      return RIGL_ERR_UNSUPPORTED;
-    }
     CUtensorMap rmap = omap;
     if (bn_apply->residual) {            // the residual through the output's view: same boxes, same swizzle
       rc = make_act_map(&rmap, bn_apply->residual, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
@@ -1087,8 +988,8 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
       return halo_launch_kmajor(hp, dy, g.cout, g.cout, pk + L.off_dgrad, L.cout_pad, g.cin, dx, g.x_pitch, true, s);
     }
   }
-  if (gate != nullptr && (st != 1 || !g_tma_store)) {   // one launch, bf16 TMA-store epilogue
-    set_error("gated dgrad: only the single-launch stride-1 dgrad with the TMA-store epilogue has the gate");
+  if (gate != nullptr && st != 1) {
+    set_error("gated dgrad: only the single-launch stride-1 dgrad has the gate");
     return RIGL_ERR_UNSUPPORTED;
   }
   // classes of input pixels by parity; each class is one launch over its sub-grid
@@ -1119,10 +1020,6 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
       set_pixel_tiling(p, gw, gh, g.batch, 128);
       p.kblks = (g.cout + kBK - 1) / kBK;
       p.N = g.cin;
-      p.out_bf16 = static_cast<__nv_bfloat16*>(dx);
-      p.o_off = ((long long)ph * g.in_w + pw) * g.x_pitch;
-      p.o_sw = (long long)st * g.x_pitch; p.o_sh = (long long)st * g.in_w * g.x_pitch;
-      p.o_sn = (long long)g.in_h * g.in_w * g.x_pitch;
       // survivor table indexed [tap][co/64][ci/64]: here N = ci, K = co
       p.nnz = reinterpret_cast<const uint32_t*>(pk + L.off_nnz);
       p.nnz_tap_stride = L.n_tiles * L.k_tiles; p.nnz_n_stride = 1; p.nnz_k_stride = L.k_tiles;
@@ -1135,15 +1032,13 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
       CUtensorMap bmap;
       const uint64_t bdims[3] = {(uint64_t)L.cout_pad, (uint64_t)g.cin, (uint64_t)g.taps()};
       const uint64_t bstr[2] = {(uint64_t)L.cout_pad * 2, (uint64_t)g.cin * L.cout_pad * 2};
-      const uint32_t bbox[3] = {(uint32_t)kBK, (uint32_t)kmajor_b_rows(p, bn_tile), 1};
+      const uint32_t bbox[3] = {(uint32_t)kBK, (uint32_t)bn_tile, 1};
       rc = make_tmap(&bmap, pk + L.off_dgrad, 3, bdims, bstr, bbox);
       if (rc != RIGL_OK) return rc;
-      CUtensorMap omap = bmap;
-      p.tma_store = g_tma_store ? 1 : 0;
-      if (p.tma_store) {                 // dx viewed through the parity sub-grid of this launch
-        rc = make_act_map(&omap, dx, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
-        if (rc != RIGL_OK) return rc;
-      }
+      CUtensorMap omap;                  // dx viewed through the parity sub-grid of this launch
+      rc = make_act_map(&omap, dx, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
+      if (rc != RIGL_OK) return rc;
+      p.tma_store = 1;
       if (gate != nullptr) {            // x through dx's view: the gate box is the output box
         CUtensorMap xmap;
         rc = make_act_map(&xmap, gate, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
@@ -1158,30 +1053,20 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
   return RIGL_OK;
 }
 
-template <int BN, int STAGES, int CL>
-static int launch_wgrad_cl(const TMaps4& xmaps, const CUtensorMap& dymap, const WgradParams& p, cudaStream_t s) {
+template <int BN, int STAGES>
+static int launch_wgrad(const TMaps4& xmaps, const CUtensorMap& dymap, const WgradParams& p, cudaStream_t s) {
   constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 1024 + 256;
   static_assert(smem <= 227 * 1024, "wgrad kernel exceeds the shared memory of an SM");
   static bool configured = false;
   if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_wgrad<BN, STAGES, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_wgrad<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  const int groups = ((p.ntaps * p.m_tiles + CL - 1) / CL) * p.n_tiles * p.splits;
-  int clusters = g_num_sms / CL;
-  if (groups < clusters) clusters = groups;
-  const int rc = launch_clustered<CL>(k_igemm_wgrad<BN, STAGES, CL>, clusters * CL, smem, s, xmaps, dymap, p);
-  if (rc != RIGL_OK) return rc;
+  const int units = p.ntaps * p.m_tiles * p.n_tiles * p.splits;
+  const int grid = units < g_num_sms ? units : g_num_sms;
+  k_igemm_wgrad<BN, STAGES><<<grid, kThreads, smem, s>>>(xmaps, dymap, p);
   RIGL_LAUNCH_CHECK("k_igemm_wgrad");
   return RIGL_OK;
-}
-
-template <int BN, int STAGES>
-static int launch_wgrad(const TMaps4& xmaps, const CUtensorMap& dymap, const WgradParams& p, cudaStream_t s) {
-  if constexpr (BN >= 128) {
-    if (g_cluster_mc && p.ntaps * p.m_tiles >= 2) return launch_wgrad_cl<BN, STAGES, 2>(xmaps, dymap, p, s);
-  }
-  return launch_wgrad_cl<BN, STAGES, 1>(xmaps, dymap, p, s);
 }
 
 int tc_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float beta, void* ws, size_t ws_bytes,

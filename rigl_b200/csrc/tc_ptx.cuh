@@ -64,46 +64,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   } while (!done);
 }
 
-// ---- clusters ---------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {       // every thread of every CTA of the cluster
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Arrive (no tx) on the barrier at the same shared-memory offset in CTA `cta` of the cluster, with cluster-scope
-// release: this thread's (and, after a wgmma wait, its warpgroup's) reads of that slot are ordered before it.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-// mbar_wait with cluster-scope acquire: the arrivals came from other CTAs of the cluster.
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  uint32_t spins = 0;
-  long long t0 = 0;
-  do {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (!done && (++spins & 0xFFFu) == 0) {
-      const long long now = clock64();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > 8000000000ll) __trap();
-    }
-  } while (!done);
-}
-
 // ---- TMA ----------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -120,23 +80,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-
-// Multicast variants: the box is written at the same CTA-relative smem offset of every CTA in
-// `mask`, and complete_tx is signalled on the mbarrier at the same offset in each of them.
-__device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
-                                               int c2, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_mc(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1,
-                                               int c2, int c3, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(mask)
       : "memory");
 }
 

@@ -559,7 +559,7 @@ class SparseConv2d(_MaskedLayer):
 
   def _fprop_bn(self, x, bn, residual):
     """conv + `bn`'s inference form (+ residual, ReLU) in one launch; None where the layer's kernel has no such
-    epilogue (RIGL_ERR_UNSUPPORTED: the patch-matrix and halo layers, RIGL_FORCE_SIMT, RIGL_TMA_STORE=0)."""
+    epilogue (RIGL_ERR_UNSUPPORTED: the patch-matrix and halo layers, RIGL_FORCE_SIMT)."""
     if self.patch_mode:
       return None
     n, c, h, w = x.shape

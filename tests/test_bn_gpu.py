@@ -217,14 +217,6 @@ def test_conv_epilogue_bn_stats_match_stats_pass(case):
   assert float((a - b).abs().max()) <= 2 ** -7 * float(b.abs().max()) + 1e-3
 
 
-def test_conv_epilogue_bn_stats_with_cluster_multicast():
-  """The statistics epilogue in the 2-CTA multicast kernels (RIGL_CLUSTER_MC=1, read once per process)."""
-  cases = [_BN_STATS_CASES[1], _BN_STATS_CASES[-2]]
-  calls = [('test_conv_epilogue_bn_stats_match_stats_pass', (c,)) for c in cases]
-  for case, ran in zip(cases, run_isolated('test_bn_gpu', calls, {'RIGL_CLUSTER_MC': '1'})):
-    assert_ran(ran, r'k_igemm_kmajor<\d+, ?\d+, ?2>', case)
-
-
 def test_conv_epilogue_bn_stats_only_where_profitable():
   """Default policy: short reductions with wide outputs (epilogue-bound layers) keep the separate stats pass."""
   from rigl_b200 import layers, pruning

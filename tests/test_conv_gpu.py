@@ -64,7 +64,7 @@ CONV_CASES = [
     (2, 9, 9, 16, 16, 3, 1, 0.3, 'VALID'),
     # ragged channel counts above 64: partially valid second 64-channel slab of a 128-wide N tile (fprop cout,
     # dgrad cin), N tiles that start at channel 128 with a few channels valid, ragged K blocks; two or more M tiles
-    # in fprop and in every dgrad parity class (so the 2-CTA multicast kernels take them too)
+    # in fprop and in every dgrad parity class
     (4, 8, 8, 72, 136, 1, 1, 0.5),
     (4, 16, 16, 96, 200, 1, 2, 0.6),
     (4, 8, 8, 200, 72, 3, 1, 0.7),
@@ -72,7 +72,6 @@ CONV_CASES = [
     (3, 7, 7, 72, 72, 3, 1, 0.5),
     (4, 11, 11, 200, 136, 3, 2, 0.6, 'SAME'),
 ]
-RAGGED_CASES = CONV_CASES[-6:]
 
 
 def _conv_case(case, force_simt, mask=None):
@@ -218,26 +217,12 @@ def test_conv_stem_patch_matrix_path(case):
     layers.STEM_S2D_PATH = old
 
 
-_MC = {'RIGL_CLUSTER_MC': '1'}
 _KMAJOR = r'k_igemm_kmajor<'
-_KMAJOR_MC = r'k_igemm_kmajor<\d+, ?\d+, ?2>'
-_KMAJOR_MC64 = r'k_igemm_kmajor<64, ?7, ?2>'
-_WGRAD_MC = r'k_igemm_wgrad<\d+, ?\d+, ?2>'
 
 
 def _isolated(calls, env, timeout=300):
   """run_isolated over this module's case functions."""
   return run_isolated('test_conv_gpu', calls, env, timeout)
-
-
-@pytest.mark.parametrize('case', [CONV_CASES[5], CONV_CASES[8], CONV_CASES[10], CONV_CASES[11]])
-def test_conv_cluster_multicast_path(case):
-  """Same results with the 2-CTA multicast clusters (RIGL_CLUSTER_MC=1, read once per process)."""
-  ran, = _isolated([('_conv_case', (case, False))], _MC)
-  if case[3] % 8 == 0:                     # (the 3-channel stem runs on its own kernels)
-    assert_ran(ran, _KMAJOR_MC, case)
-  if case[4] >= 128:                       # 128-wide wgrad N tiles: the dY tile is multicast
-    assert_ran(ran, _WGRAD_MC, case)
 
 
 # 3x3 / stride 1 / pad 1 layers with <= 64 reduction channels run on the halo kernels (one halo tile in
@@ -433,41 +418,22 @@ def test_depthwise3x3_vs_fp64(case):
 # ---- dead weight tiles (tile_masks.py): the survivor-table lookups that let the K-major kernels skip the load and
 # the MMA of an all-zero 64x64 weight tile.  Run in a child process with a time limit, because a producer and
 # consumers that disagree on which K blocks are live would wait on each other forever.
-@pytest.mark.parametrize('env', [{}, _MC], ids=['default', 'cluster_mc'])
+@pytest.mark.parametrize('env', [{}], ids=['default'])
 def test_conv_dead_weight_tiles(env):
   ran = _isolated([('_conv_case', (case, False, pattern)) for case, pattern in STRUCTURED_CONV_CASES], env, 600)
   for (case, pattern), names in zip(STRUCTURED_CONV_CASES, ran):
     if case[3] <= 64 and case[6] == 1:      # the halo case: its kernels keep all nine taps' weights resident
       assert_ran(names, r'k_halo3x3_kmajor', (case, pattern))
     else:
-      assert_ran(names, _KMAJOR_MC if env else _KMAJOR, (case, pattern))
+      assert_ran(names, _KMAJOR, (case, pattern))
 
 
-@pytest.mark.parametrize('env', [{}, _MC], ids=['default', 'cluster_mc'])
+@pytest.mark.parametrize('env', [{}], ids=['default'])
 def test_linear_dead_weight_tiles_at_the_liveness_cap(env):
   """K = 320 blocks (dead blocks skipped) and 321 blocks (every block loaded) in fprop and in dgrad."""
   calls = [('_linear_case', (case, False, 'f32', True, pattern)) for case, pattern in STRUCTURED_LINEAR_CASES]
   for (case, pattern), names in zip(STRUCTURED_LINEAR_CASES, _isolated(calls, env, 600)):
-    assert_ran(names, _KMAJOR_MC if env else _KMAJOR, (case, pattern))
-
-
-@pytest.mark.parametrize('env', [_MC, {'RIGL_TMA_STORE': '0'}], ids=['cluster_mc', 'tma_store_0'])
-def test_conv_ragged_channels_variants(env):
-  """The ragged channel counts (in-process under the default environment: CONV_CASES) with the 2-CTA multicast and
-  with RIGL_TMA_STORE=0, the per-thread bf16 stores (fprop, and dgrad through the stride-2 parity offsets); plus a
-  bf16 linear layer without a bias (TMA store by default)."""
-  calls = [('_conv_case', (c, False)) for c in RAGGED_CASES] + \
-      [('_linear_case', ((130, 200, 200, 0.6), False, 'bf16', False))]
-  for case, names in zip(RAGGED_CASES + [None], _isolated(calls, env)):
-    assert_ran(names, _KMAJOR_MC if 'RIGL_CLUSTER_MC' in env else _KMAJOR, case)
-
-
-def test_conv_cluster_multicast_64_wide_odd_m_tiles():
-  """3 M tiles (16x8x1-pixel boxes): the partner of the last tile lies past the grid.  64-wide N tiles in
-  multicast mode: fprop of the first case, dgrad of the second."""
-  cases = [(3, 8, 16, 128, 64, 1, 1, 0.5), (3, 8, 16, 64, 256, 1, 1, 0.5)]
-  for case, ran in zip(cases, _isolated([('_conv_case', (c, False)) for c in cases], _MC)):
-    assert_ran(ran, _KMAJOR_MC64, case)
+    assert_ran(names, _KMAJOR, (case, pattern))
 
 
 def _packed_layout(taps, cin, cout):

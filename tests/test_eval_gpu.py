@@ -12,7 +12,7 @@ from rigl_b200.evaluate import Evaluator
 from rigl_b200.layers import SparseConv2d, _workspace
 from rigl_b200.norm import FusedBatchNormReLU
 
-from isolated import assert_not_ran, assert_ran, run_isolated
+from isolated import assert_not_ran, assert_ran
 from tile_masks import tile_mask
 
 pytestmark = pytest.mark.gpu
@@ -328,29 +328,3 @@ def test_eval_once_after_restore_matches_the_original():
   l = model.registry.layers()[5]
   assert got['pruning/%s/mask/sparsity' % l.scope] == pytest.approx(l.mask.sparsity())
 
-
-# ---- variants selected by environment switches (child processes) ----
-def child_bnapply_cases():
-  for cin, cout, k, s, h, res in ((256, 64, 1, 1, 9, True), (64, 256, 1, 1, 7, True), (128, 128, 3, 2, 14, False),
-                                  (512, 320, 1, 1, 5, True)):
-    rc, out, ref = _compare(cin, cout, k, s, h, batch=3, residual=res)
-    assert rc == 0, _cabi.lib().rigl_last_error()
-    assert torch.equal(out, ref), (cin, cout, k, s, h, res)
-
-
-def child_bnapply_unsupported():
-  rc, _, _ = _compare(256, 64, 1, 1, 9)
-  assert rc == -4, rc
-  model = _build('mobilenet_v2', seed=8)
-  x = _images(2, 64, 50)
-  assert torch.equal(_eval_logits(model, x, True), _eval_logits(model, x, False))
-
-
-def test_bnapply_cluster_multicast_variant():
-  ran = run_isolated('test_eval_gpu', [('child_bnapply_cases', ())], env={'RIGL_CLUSTER_MC': '1'})
-  assert_ran(ran[0], r'k_igemm_kmajor_bn<\d+, ?\d+, ?2>', 'RIGL_CLUSTER_MC=1')
-
-
-def test_bnapply_unsupported_without_tma_store():
-  ran = run_isolated('test_eval_gpu', [('child_bnapply_unsupported', ())], env={'RIGL_TMA_STORE': '0'})
-  assert_not_ran(ran[0], _BN_KERNEL, 'RIGL_TMA_STORE=0')

@@ -62,8 +62,7 @@ def tile_mask(pattern, shape, rng, sparsity=0.5):
 
 # (n, h, w, cin, cout, k, stride, sparsity inside live tiles[, padding]), pattern.  Channel counts > 64 (or a
 # stride of 2) keep 3x3 layers off the halo kernels, which ignore the table -- except the last case, which is a
-# halo layer on purpose.  n and the pixel grids give two or more 128-pixel M tiles, so the 2-CTA multicast kernels
-# run on them too.
+# halo layer on purpose.  n and the pixel grids give two or more 128-pixel M tiles.
 STRUCTURED_CONV_CASES = [
     ((3, 8, 8, 192, 320, 3, 1, 0.5), 'staircase'),        # 3 vs 5 tile counts; the last 128-wide N tile is half past N
     ((3, 8, 8, 320, 192, 3, 1, 0.5), 'staircase'),

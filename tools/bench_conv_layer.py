@@ -3,7 +3,7 @@ same host calls the training step makes.  One JSON line per (shape, op): microse
 events, median of --iters, inputs rotated through buffers larger than L2), dense-executed TFLOP/s
 and algorithmic GB/s.  `fprop_stats` is the fprop with the batch-norm statistics epilogue, run for every shape
 (rigl_set_bn_stats_always), not only where the training step would use it.  Kernel-selection switches
-(RIGL_HALO3X3, RIGL_TMA_STORE ...) are read once per process: run one process per configuration.
+(RIGL_HALO3X3, RIGL_FORCE_SIMT ...) are read once per process: run one process per configuration.
 
   python tools/bench_conv_layer.py [--shapes r50s1] [--iters 20] [--tag name]
 """
