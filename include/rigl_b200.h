@@ -140,6 +140,20 @@ RIGL_API int rigl_mask_update_run(rigl_mask_plan* plan, float drop_fraction, int
 RIGL_API int rigl_mask_update_run_noise(rigl_mask_plan* plan, float drop_fraction, int grow_mode,
                          float grow_divisor, float acc_scale, int reinit_when_same, float noise_std,
                          uint64_t noise_seed, void* workspace, size_t workspace_bytes, void* stream);
+/* Gradual magnitude pruning (Zhu & Gupta): one threshold update of every layer.  Replaces
+ * tensorflow.contrib.model_pruning's Pruning.conditional_mask_update_op / _get_mask_assign_ops (the `prune`
+ * method of cifar_resnet/resnet_train_eval.py:249-275 and mnist/mnist_train_eval.py:320-335).  Every layer of the
+ * plan must be RIGL_LAYER_DROP_ONLY | RIGL_LAYER_ALL_ACTIVE with no score_drop and no noise; keep[l] (host array,
+ * 1 <= keep[l] <= n) is the layer's k for this update and becomes its n_prune_override = n - k (it stays in the
+ * plan: a later rigl_mask_update_run on the same plan would use it).  Per layer:
+ *   cur = the k-th largest |w| (-0.0 counts as 0)
+ *   thr = f32(f32(cur * f32(1 - threshold_decay)) + f32(old_thr[l] * threshold_decay))    (no FMA)
+ *   new_thr[l] <- thr;  mask <- |w| >= thr (every tie at thr is kept); weights and slots are not touched.
+ * old_thr / new_thr: [n_layers] float32 on the device, may be the same array.  Stream-ordered kernel launches only
+ * (the keep counts travel as kernel arguments, no copy from host memory), so the call never waits for the device;
+ * 7 launches + 1 memset for up to 2048 layers, one more launch per further 2048. */
+RIGL_API int rigl_mask_prune_run(rigl_mask_plan* plan, const int32_t* keep, const float* old_thr, float* new_thr,
+                         float threshold_decay, void* workspace, size_t workspace_bytes, void* stream);
 /* out[i] <- exactly the noise rigl_mask_update_run_noise adds to element i of a layer with this key
  * (tests and the CPU oracle consume it; the product path never materialises it). */
 RIGL_API int rigl_mask_noise_fill(float* out, int64_t n, uint32_t layer_noise_key, float noise_std,

@@ -14,7 +14,7 @@ _lib = None
 # residual form without a ReLU bitmap when relu == 0 (the linear bottleneck of MobileNet-v2).  Library version 203
 # only adds rigl_masked_conv2d_fprop_bnapply; no calling rule of an existing symbol changed, and a library without
 # the new symbol already fails its lookup in lib().  204 only adds the ReLU entry points (conv epilogues, the 2x2
-# pool, rigl_relu_gate), likewise.
+# pool, rigl_relu_gate), likewise; 205 only adds rigl_mask_prune_run.
 ABI_VERSION = 202
 
 
@@ -70,6 +70,7 @@ SIGNATURES = {
     'rigl_mask_plan_workspace_bytes': (_sz, [_vp]),
     'rigl_mask_update_run': (C.c_int, [_vp, _f32, _i32, _f32, _f32, _i32, _vp, _sz, _vp]),
     'rigl_mask_update_run_noise': (C.c_int, [_vp, _f32, _i32, _f32, _f32, _i32, _f32, C.c_uint64, _vp, _sz, _vp]),
+    'rigl_mask_prune_run': (C.c_int, [_vp, C.POINTER(C.c_int32), _vp, _vp, _f32, _vp, _sz, _vp]),
     'rigl_mask_noise_fill': (C.c_int, [_vp, _i64, C.c_uint32, _f32, C.c_uint64, _vp]),
     'rigl_mask_plan_read_stats': (C.c_int, [_vp, _vp, C.POINTER(C.c_int32), _vp]),
     'rigl_packed_weights_bytes': (_sz, [_i32, _i32, _i32]),

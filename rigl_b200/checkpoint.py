@@ -41,7 +41,7 @@ def _scalar_handle(get, set_):
   return Handle(lambda: np.asarray(get(), dtype=np.float64), lambda a: set_(np.asarray(a).reshape(-1)[0]))
 
 
-def variables_of(model, optimizer=None, sparse_optimizer=None, ckpt_path=None):
+def variables_of(model, optimizer=None, sparse_optimizer=None, ckpt_path=None, pruning=None):
   """OrderedDict name -> Handle for a rigl_b200 model: masks, masked weights, the remaining
   parameters / buffers, (optionally) the inner optimizer's per-parameter state tensors and the sparse
   optimizer's own state.
@@ -52,6 +52,8 @@ def variables_of(model, optimizer=None, sparse_optimizer=None, ckpt_path=None):
     (sparse_optimizers_base.py:166-171), so it lives in its checkpoints; without it a resumed run would
     re-initialise it to -frequency and fire an off-schedule mask update -- and, for
     SparseMomentumOptimizer, the EMA shadows `<scope>/weights/ExponentialMovingAverage`.
+  pruning: a pruning.Pruning; adds every layer's `<scope>/threshold` and `<name>/last_mask_update_step`
+    (e.g. `model_pruning/last_mask_update_step`), the variables contrib's Pruning keeps in its checkpoints.
   ckpt_path: a checkpoint about to be restored.  A freshly built torch optimizer has an EMPTY state, so
     its slots (`<scope>/weights/momentum_buffer` ...) would be skipped silently; every slot the file holds
     for a known parameter is materialised (zeros) in `optimizer.state` here so that restore() fills it."""
@@ -96,6 +98,11 @@ def variables_of(model, optimizer=None, sparse_optimizer=None, ckpt_path=None):
         if name not in so._ema:
           so._ema[name] = torch.zeros(l.weight.numel(), dtype=torch.float32, device=l.weight.device)
         out[l.scope + '/weights/ExponentialMovingAverage'] = _tensor_handle(so._ema[name])
+  if pruning is not None:
+    for l in model.registry.layers():
+      out[l.scope + '/threshold'] = _tensor_handle(l.threshold)
+    out[pruning.spec.name + '/last_mask_update_step'] = _scalar_handle(
+        lambda: pruning.last_update_step, lambda v: setattr(pruning, 'last_update_step', int(v)))
   return out
 
 

@@ -66,7 +66,7 @@ __global__ void k_apply_mask_f32(const float* __restrict__ src, const uint32_t* 
 
 using namespace rigl;
 
-extern "C" int rigl_version(void) { return 204; }
+extern "C" int rigl_version(void) { return 205; }
 extern "C" const char* rigl_last_error(void) { return g_err; }
 extern "C" uint64_t rigl_launch_count(void) { return g_launches.load(); }
 

@@ -36,6 +36,7 @@
 // blocks; measured 0.36 -> 0.30 ms for the sequence).  Cutting the shared-memory
 // histogram atomics 8x (a sampled floor under the grow threshold, validated in-kernel)
 // was built and measured: 125 -> 112 us for C, paid back by the sampling -- not kept.
+#include <algorithm>
 #include <cstdlib>
 #include <vector>
 
@@ -758,6 +759,80 @@ k_scan_grow(const LayerDev* __restrict__ layers, const BlockTask* __restrict__ t
 }
 
 // ----------------------------------------------------------------------------
+// Gradual magnitude pruning (rigl_mask_prune_run): A-D with DROP_ONLY | ALL_ACTIVE and n_keep = k select the top k
+// of |w|; these two kernels turn that cut into contrib's threshold and mask = |w| >= threshold (ties kept).
+// ----------------------------------------------------------------------------
+__device__ __forceinline__ float key_to_float(uint32_t key) {
+  return __uint_as_float((key & 0x80000000u) ? (key ^ 0x80000000u) : ~key);
+}
+
+// Writes n_prune_override = n - k of up to kPruneCountBatch layers into the device layer table, from the kernel
+// arguments (8 KB of parameters: CUDA 12.1+ on sm_70+ allows up to 32 KB).
+constexpr int kPruneCountBatch = 2048;
+struct PruneCounts {
+  int32_t n_prune[kPruneCountBatch];
+};
+
+__global__ void k_prune_set_counts(LayerDev* __restrict__ layers, int first, int count, const PruneCounts counts) {
+  for (int i = threadIdx.x; i < count; i += blockDim.x) layers[first + i].n_prune_override = counts.n_prune[i];
+}
+
+// H: per layer (one block): cur = the k-th largest |w| = the smallest key D kept.  Every kept position outside the
+// drop threshold bin lies above it, and k >= 1 keeps at least one candidate of that bin, so the minimum over the
+// kept candidates is the cut.  thr = cur * (1 - decay) + old * decay, each product and the sum rounded (no FMA).
+__global__ void __launch_bounds__(kScanThreads)
+k_prune_threshold(const LayerDev* __restrict__ layers, const uint8_t* __restrict__ ws, const float* old_thr,
+                  float* new_thr, float decay) {      // (old_thr may alias new_thr)
+  __shared__ uint32_t s_min;
+  const LayerDev L = layers[blockIdx.x];
+  const LayerState* st = reinterpret_cast<const LayerState*>(ws + L.off_state);
+  const uint32_t* mask1 = reinterpret_cast<const uint32_t*>(ws + L.off_mask1);
+  const uint2* cand = reinterpret_cast<const uint2*>(ws + L.off_cand);
+  if (threadIdx.x == 0) s_min = 0xFFFFFFFFu;
+  __syncthreads();
+  const uint32_t cnt = st->cand_cnt_drop;
+  uint32_t m = 0xFFFFFFFFu;
+  for (uint32_t i = threadIdx.x; i < cnt; i += kScanThreads) {
+    const uint2 c = cand[i];
+    if ((__ldcg(mask1 + (c.y >> 5)) >> (c.y & 31)) & 1u) m = min(m, c.x);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = min(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMin(&s_min, m);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const float cur = key_to_float(s_min);
+    new_thr[blockIdx.x] = __fadd_rn(__fmul_rn(cur, __fsub_rn(1.0f, decay)), __fmul_rn(old_thr[blockIdx.x], decay));
+  }
+}
+
+// P: every scan block rewrites its chunk of the layer's bitmap as |w| >= thr.  All layers, full grid.
+__global__ void __launch_bounds__(kScanThreads)
+k_prune_publish(const LayerDev* __restrict__ layers, const BlockTask* __restrict__ tasks, const float* __restrict__ thr,
+                RunParams prm) {
+  const BlockTask task = tasks[blockIdx.x];
+  const LayerDev L = layers[task.layer];
+  const float t = thr[task.layer];
+  const uint32_t n = L.n, words = (n + 31) >> 5;
+  const uint32_t end = min(n, task.start + prm.chunk);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int kWarps = kScanThreads / 32;
+#pragma unroll 4
+  for (uint32_t base = task.start + (uint32_t)warp * kGroup; base < end; base += kWarps * kGroup) {
+    const uint32_t e0 = base + 4 * lane;
+    const float4 v = load4_guard(L.w, e0, n);
+    const float ws4[4] = {v.x, v.y, v.z, v.w};
+    uint32_t nib = 0;
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+      if (e0 + c < n && fabsf(ws4[c]) >= t) nib |= 1u << c;
+    const uint32_t word = combine_nibbles(nib, lane);
+    const uint32_t widx = (base >> 5) + (lane >> 3);
+    if ((lane & 7) == 0 && widx < words) L.mask[widx] = word;
+  }
+}
+
+// ----------------------------------------------------------------------------
 // Host side: plan
 // ----------------------------------------------------------------------------
 }  // namespace rigl
@@ -772,6 +847,7 @@ struct rigl_mask_plan {
   size_t state_off = 0;
   size_t task_cnt_off = 0; // [n_blocks] grow candidates per scan block
   int chunk = rigl::kChunk; // elements per scan block
+  std::vector<rigl::LayerDev> h_layers;   // host copy of d_layers (rigl_mask_prune_run validates against it)
 };
 
 using namespace rigl;
@@ -840,6 +916,7 @@ extern "C" int rigl_mask_plan_create(const rigl_layer_desc* layers, int n_layers
   p->state_off = state_off;
   p->task_cnt_off = task_cnt_off;
   p->chunk = (int)chunk;
+  p->h_layers = host;
   cudaError_t e = cudaMalloc(&p->d_layers, sizeof(LayerDev) * n_layers);
   if (e == cudaSuccess) e = cudaMalloc(&p->d_tasks, sizeof(BlockTask) * tasks.size());
   if (e == cudaSuccess) e = cudaMemcpy(p->d_layers, host.data(), sizeof(LayerDev) * n_layers, cudaMemcpyHostToDevice);
@@ -864,20 +941,18 @@ extern "C" size_t rigl_mask_plan_workspace_bytes(const rigl_mask_plan* plan) {
   return plan ? plan->ws_bytes : 0;
 }
 
-static int mask_update_launch(rigl_mask_plan* plan, const RunParams& prm_, void* workspace, size_t workspace_bytes,
-                              void* stream_) {
-  RunParams prm = prm_;
+static int check_workspace(const rigl_mask_plan* plan, const void* workspace, size_t workspace_bytes) {
   RIGL_REQUIRE(plan && workspace, "rigl_mask_update_run: null plan/workspace");
   if (workspace_bytes < plan->ws_bytes) {
     set_error("rigl_mask_update_run: workspace %zu < required %zu", workspace_bytes, plan->ws_bytes);
     return RIGL_ERR_WORKSPACE;
   }
   RIGL_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "workspace must be 256B aligned");
-  RIGL_REQUIRE(prm.grow_mode >= RIGL_GROW_ZEROS && prm.grow_mode <= RIGL_GROW_GRAD_SIGN, "bad grow_mode %d", prm.grow_mode);
-  RIGL_REQUIRE(prm.drop_fraction >= 0.f && prm.drop_fraction <= 1.f, "drop_fraction %f outside [0,1]", prm.drop_fraction);
-  RIGL_REQUIRE(prm.noise_std >= 0.f, "noise_std must be >= 0");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  return RIGL_OK;
+}
+
+// zero the workspace's state region, then A-D: the drop cut of every layer (mask1 = the kept set)
+static int launch_drop_select(rigl_mask_plan* plan, RunParams& prm, uint8_t* ws, cudaStream_t stream) {
   RIGL_CUDA(cudaMemsetAsync(ws, 0, plan->zero_bytes, stream));
   prm.off_task_cnt = plan->task_cnt_off;
   prm.n_blocks = (uint32_t)plan->n_blocks;
@@ -893,6 +968,19 @@ static int mask_update_launch(rigl_mask_plan* plan, const RunParams& prm_, void*
   RIGL_LAUNCH_CHECK("k_scan_drop");
   k_resolve<false><<<plan->n_layers, kResolveThreads, 0, stream>>>(plan->d_layers, ws, prm);
   RIGL_LAUNCH_CHECK("k_resolve<drop>");
+  return RIGL_OK;
+}
+
+static int mask_update_launch(rigl_mask_plan* plan, const RunParams& prm_, void* workspace, size_t workspace_bytes,
+                              void* stream_) {
+  RunParams prm = prm_;
+  if (int rc = check_workspace(plan, workspace, workspace_bytes)) return rc;
+  RIGL_REQUIRE(prm.grow_mode >= RIGL_GROW_ZEROS && prm.grow_mode <= RIGL_GROW_GRAD_SIGN, "bad grow_mode %d", prm.grow_mode);
+  RIGL_REQUIRE(prm.drop_fraction >= 0.f && prm.drop_fraction <= 1.f, "drop_fraction %f outside [0,1]", prm.drop_fraction);
+  RIGL_REQUIRE(prm.noise_std >= 0.f, "noise_std must be >= 0");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  if (int rc = launch_drop_select(plan, prm, ws, stream)) return rc;
   k_scan_grow<<<plan->n_blocks, kScanThreads, 0, stream>>>(plan->d_layers, plan->d_tasks, ws, prm);
   RIGL_LAUNCH_CHECK("k_scan_grow");
   k_resolve<true><<<plan->n_layers, kResolveThreads, 0, stream>>>(plan->d_layers, ws, prm);
@@ -916,6 +1004,38 @@ extern "C" int rigl_mask_update_run_noise(rigl_mask_plan* plan, float drop_fract
   RunParams prm{drop_fraction, grow_mode, grow_divisor, acc_scale, reinit_when_same, noise_std,
                 (uint32_t)(noise_seed & 0xffffffffu), (uint32_t)(noise_seed >> 32), 0ull, 0u, 0u};
   return mask_update_launch(plan, prm, workspace, workspace_bytes, stream_);
+}
+
+extern "C" int rigl_mask_prune_run(rigl_mask_plan* plan, const int32_t* keep, const float* old_thr, float* new_thr,
+                                   float threshold_decay, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int rc = check_workspace(plan, workspace, workspace_bytes)) return rc;
+  RIGL_REQUIRE(keep && old_thr && new_thr, "rigl_mask_prune_run: null keep/old_thr/new_thr");
+  RIGL_REQUIRE(threshold_decay >= 0.f && threshold_decay <= 1.f, "threshold_decay %f outside [0,1]", threshold_decay);
+  for (int l = 0; l < plan->n_layers; ++l) {
+    const LayerDev& L = plan->h_layers[l];
+    RIGL_REQUIRE((L.flags & (RIGL_LAYER_DROP_ONLY | RIGL_LAYER_ALL_ACTIVE)) == (RIGL_LAYER_DROP_ONLY | RIGL_LAYER_ALL_ACTIVE)
+                     && !L.sdrop && !L.noise,
+                 "rigl_mask_prune_run: layer %d needs DROP_ONLY | ALL_ACTIVE, no score_drop and no noise", l);
+    RIGL_REQUIRE(keep[l] >= 1 && (uint32_t)keep[l] <= L.n, "rigl_mask_prune_run: layer %d keeps %d of %u", l, keep[l],
+                 L.n);
+  }
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // the counts travel as kernel arguments: no copy from host memory, so nothing can wait for the device
+  for (int first = 0; first < plan->n_layers; first += kPruneCountBatch) {
+    PruneCounts c;
+    const int count = std::min(kPruneCountBatch, plan->n_layers - first);
+    for (int i = 0; i < count; ++i) c.n_prune[i] = (int32_t)plan->h_layers[first + i].n - keep[first + i];
+    k_prune_set_counts<<<1, kScanThreads, 0, stream>>>(plan->d_layers, first, count, c);
+    RIGL_LAUNCH_CHECK("k_prune_set_counts");
+  }
+  RunParams prm{0.f, RIGL_GROW_ZEROS, 1.f, 0.f, 0, 0.f, 0u, 0u, 0ull, 0u, 0u};
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  if (int rc = launch_drop_select(plan, prm, ws, stream)) return rc;
+  k_prune_threshold<<<plan->n_layers, kScanThreads, 0, stream>>>(plan->d_layers, ws, old_thr, new_thr, threshold_decay);
+  RIGL_LAUNCH_CHECK("k_prune_threshold");
+  k_prune_publish<<<plan->n_blocks, kScanThreads, 0, stream>>>(plan->d_layers, plan->d_tasks, new_thr, prm);
+  RIGL_LAUNCH_CHECK("k_prune_publish");
+  return RIGL_OK;
 }
 
 extern "C" int rigl_mask_noise_fill(float* out, int64_t n, uint32_t layer_noise_key, float noise_std,

@@ -327,6 +327,9 @@ class _MaskedLayer(nn.Module):
     self.weight.name = scope + '/weights:0'
     self.mask = MaskVariable(scope, shape_hwio, device)
     self.masked_weights = MaskedWeights(scope, w.numel(), device)
+    # contrib's `<scope>/threshold` variable (gradual magnitude pruning); pruning.Pruning rebinds it to a view of
+    # one flat tensor shared by every layer
+    self.threshold = torch.zeros((), dtype=torch.float32, device=device)
     taps = int(np.prod(shape_hwio[:-2])) if len(shape_hwio) > 2 else 1
     self._taps, self._cin, self._cout = taps, int(shape_hwio[-2]), int(shape_hwio[-1])
     nbytes = int(_cabi.lib().rigl_packed_weights_bytes(taps, self._cin, self._cout))

@@ -205,6 +205,19 @@ class MaskUpdateEngine(object):
         int(bool(reinit_when_same)), self._ws.data_ptr(), self._ws.numel(), _cabi.stream_ptr()),
                 'rigl_mask_update_run')
 
+  def prune(self, layers, keep, thresholds, threshold_decay):
+    """Gradual magnitude pruning of every layer (rigl_mask_prune_run): layers as for `run`, each with flags
+    LAYER_DROP_ONLY | LAYER_ALL_ACTIVE; keep[l] = the layer's k; thresholds: float32 [n_layers] on the device, read
+    as the old thresholds and overwritten with the new ones.  Asynchronous on the current stream."""
+    self.prepare(layers)
+    if (thresholds.dtype != torch.float32 or not thresholds.is_contiguous() or thresholds.numel() != len(layers)
+        or not thresholds.is_cuda):
+      raise ValueError('thresholds must be a contiguous float32 CUDA tensor of %d elements' % len(layers))
+    k = (C.c_int32 * len(layers))(*[int(v) for v in keep])
+    _cabi.check(_cabi.lib().rigl_mask_prune_run(self._plan, k, thresholds.data_ptr(), thresholds.data_ptr(),
+                                                float(threshold_decay), self._ws.data_ptr(), self._ws.numel(),
+                                                _cabi.stream_ptr()), 'rigl_mask_prune_run')
+
   def stats(self):
     """[(n_ones, n_prune, n_keep, drop_candidates, grow_candidates, drop_bin, grow_bin)] per layer."""
     out = (C.c_int32 * (8 * self._n_layers))()

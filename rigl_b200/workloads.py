@@ -454,14 +454,17 @@ class TrainHarness(object):
   def __init__(self, model, lr=0.1, momentum=0.9, weight_decay=1e-4, label_smoothing=0.1,
                drop_fraction=0.3, drop_fraction_anneal='cosine', begin_step=0, end_step=25000,
                frequency=100, data_parallel=None, optimizer_cls=SparseRigLOptimizer, lr_schedule=None,
-               fused_optimizer=None, inner_optimizer='momentum'):
+               fused_optimizer=None, inner_optimizer='momentum', pruning=None):
     """lr_schedule: optional callable(global_step) -> learning rate, evaluated on the host before every step
     (optim.make_imagenet_lr_fn is the reference's, imagenet_train_eval.py:317-354); `lr` is then only the
     initial value.  fused_optimizer: the inner optimizer is optim.FusedMomentumSGD (one launch, mask * dense_grad
     fused in, device-resident learning rate); default on for CUDA models (RIGL_FUSED_SGD=0 -> torch.optim.SGD).
     inner_optimizer: 'momentum' (the above) or 'adam' -- optim.FusedAdam(lr, weight_decay) with TF's beta1,
     beta2 and epsilon, the reference's `--use_adam` (imagenet_train_eval.py:355-358; there the learning rate is
-    the constant base_lr * batch / 256).  'adam' exists only on the fused path: `momentum` is then unused."""
+    the constant base_lr * batch / 256).  'adam' exists only on the fused path: `momentum` is then unused.
+    optimizer_cls=None: the inner optimizer alone, one step and one global-step increment per step (the
+    reference's scratch / baseline / prune methods: `optimizer.minimize`).  pruning: a pruning.Pruning whose
+    conditional_mask_update_op() runs after every step, eager or graphed; it counts this harness's global step."""
     import os
     if inner_optimizer not in ('momentum', 'adam'):
       raise ValueError("inner_optimizer must be 'momentum' or 'adam', got %r" % (inner_optimizer,))
@@ -485,10 +488,16 @@ class TrainHarness(object):
     else:
       self.inner = torch.optim.SGD(model.parameters(), lr=lr, momentum=momentum, nesterov=True,
                                    weight_decay=weight_decay, foreach=True)
-    self.opt = optimizer_cls(self.inner, begin_step, end_step, frequency, drop_fraction=drop_fraction,
-                             drop_fraction_anneal=drop_fraction_anneal,
-                             use_tpu=data_parallel is not None).bind(model.registry)
-    self.global_step = GlobalStep(0)
+    self.opt = None if optimizer_cls is None else optimizer_cls(
+        self.inner, begin_step, end_step, frequency, drop_fraction=drop_fraction,
+        drop_fraction_anneal=drop_fraction_anneal, use_tpu=data_parallel is not None).bind(model.registry)
+    self.pruning = pruning
+    if pruning is not None and pruning.global_step is not None:
+      self.global_step = pruning.global_step
+    else:
+      self.global_step = GlobalStep(0)
+    if pruning is not None:
+      pruning.global_step = self.global_step
     self.dp = data_parallel
     # Gradient exchange under data parallelism.  Default: ONE all-reduce of the flat buffer between the two graph
     # replays (backward; optimizer).  RIGL_DP_OVERLAP=1: bucketed all-reduces launched from inside backward on a
@@ -617,14 +626,19 @@ class TrainHarness(object):
     self.replayed_kernel_launches += self.graph_kernel_launches
     if self.dp is not None and not self._dp_overlap:
       self.dp.reduce_gradients(self.model)
-    self.opt.collect_masked_grads()
     gs = self.global_step
-    self.opt._global_step = gs
-    # same decision as SparseRigLOptimizerBase.apply_gradients, with the inner step replayed
     def inner_step():
       self._g_opt.replay()
       gs.increment()
-    self.opt.cond_mask_update_op(gs, inner_step)
+    if self.opt is None:
+      inner_step()
+    else:
+      self.opt.collect_masked_grads()
+      self.opt._global_step = gs
+      # same decision as SparseRigLOptimizerBase.apply_gradients, with the inner step replayed
+      self.opt.cond_mask_update_op(gs, inner_step)
+    if self.pruning is not None:
+      self.pruning.conditional_mask_update_op()
     return self._sloss
 
   def step(self, images, labels):
@@ -637,8 +651,14 @@ class TrainHarness(object):
     loss = self._forward_backward(images, labels, set_to_none=self.dp is None)
     if self.dp is not None and not self._dp_overlap:
       self.dp.reduce_gradients(self.model)
-    self.opt.collect_masked_grads()
-    self.opt.apply_gradients(None, global_step=self.global_step)
+    if self.opt is None:
+      self.inner.step()
+      self.global_step.increment()
+    else:
+      self.opt.collect_masked_grads()
+      self.opt.apply_gradients(None, global_step=self.global_step)
+    if self.pruning is not None:
+      self.pruning.conditional_mask_update_op()
     return loss
 
 
