@@ -15,12 +15,8 @@ Layout: ONE flat fp32 buffer  [ other gradients (BN, biases) | layer 0 | layer 1
 slices).  The masked weight gradient is re-derived locally as mask * dense / world (inside the fused optimizer
 kernel), so it is never communicated.
 
-Exchange: the buffer is cut into BUCKETS of consecutive layers.  Backward produces the layers last-to-first, so
-as soon as the dense wgrad of a bucket's FIRST layer has been issued the whole bucket is complete and its SUM
-all-reduce is launched on a communication stream, overlapping the rest of the backward pass
-(`begin_backward` / `layer_done` / `finish`, driven by layers._MaskedConvFn.backward and TrainHarness).  The head
-bucket (other gradients + the first layers) goes last, after backward.  Under CUDA-graph capture the collectives
-are captured with the step (NCCL supports capture); `reduce_gradients` is the blocking one-call form.
+Exchange: after backward, ONE SUM all-reduce of the whole flat buffer (`reduce_gradients`); under CUDA graphs it
+runs eagerly between the backward replay and the optimizer replay.
 """
 import torch
 import torch.distributed as dist
@@ -32,24 +28,18 @@ def _align(n, a=128):
 
 class DataParallel(object):
 
-  def __init__(self, process_group=None, bucket_elems=6 << 20):
+  def __init__(self, process_group=None):
     if not (dist.is_available() and dist.is_initialized()):
       raise RuntimeError('torch.distributed must be initialised before DataParallel')
     self.group = process_group
     self.world = dist.get_world_size(process_group)
     self.rank = dist.get_rank(process_group)
-    self.bucket_elems = int(bucket_elems)
     self.flat = None
     self.flat_dense = None
     self.flat_other = None
     self._others = []
     self.masked_grads_in_optimizer = False   # the fused optimizer forms mask * dense / world itself
     self.other_scale_in_optimizer = False    # ... and scales the other gradients by 1 / world
-    self._buckets = []                       # (first layer index, start, stop) in the flat buffer, tail buckets first
-    self._trigger = {}                       # id(layer) -> bucket index
-    self._comm = None
-    self._pending = False
-    self.overlapped = False                  # True while a backward pass launches the bucket all-reduces itself
 
   # -- setup ------------------------------------------------------------------
   def attach(self, model):
@@ -74,71 +64,14 @@ class DataParallel(object):
       n = p.numel()
       p.grad = self.flat_other[off:off + n].view_as(p)
       off += _align(n, 4)
-    off, starts = n_other, []
+    off = n_other
     for l in layers:
       n = l.weight.numel()
       l.masked_weights.dense_grad = self.flat[off:off + n]
-      starts.append(off)
       off += _align(n)
-    # buckets of consecutive layers, built from the LAST layer backwards (the order backward finishes them)
-    self._buckets, self._trigger = [], {}
-    stop, i = total, len(layers)               # layers [first, i) form the bucket under construction
-    while i > 0:
-      first = i - 1
-      while first > 0 and (stop - starts[first]) < self.bucket_elems:
-        first -= 1
-      if first == 0:                                   # head bucket: takes the other gradients too
-        self._buckets.append((0, 0, stop))
-      else:
-        self._buckets.append((first, starts[first], stop))
-        self._trigger[id(layers[first])] = len(self._buckets) - 1
-      stop, i = starts[first], first
-    self._layers = layers
-    if dev.type == 'cuda':
-      self._comm = torch.cuda.Stream(device=dev)
     return self
 
-  # -- overlapped exchange, driven by the backward pass ---------------------------
-  def begin_backward(self):
-    self._pending = True
-    self.overlapped = True
-
-  def layer_done(self, layer, producer_stream=None):
-    """The dense wgrad of `layer` has been issued on `producer_stream` (default: the current stream).  If it is the
-    first layer of a bucket, every gradient of that bucket is now in flight: all-reduce it behind them."""
-    if not self.overlapped or self.world == 1:
-      return
-    b = self._trigger.get(id(layer))
-    if b is not None:
-      _, start, stop = self._buckets[b]
-      self._all_reduce_slice(start, stop, producer_stream)
-
-  def _all_reduce_slice(self, start, stop, producer_stream):
-    buf = self.flat[start:stop]
-    if self._comm is None:
-      dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=self.group)
-      return
-    src = producer_stream if producer_stream is not None else torch.cuda.current_stream(buf.device)
-    self._comm.wait_stream(src)
-    with torch.cuda.stream(self._comm):
-      dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=self.group)
-
-  def finish(self, model=None, producer_streams=()):
-    """After backward(): all-reduce the head bucket (other gradients + first layers), make the current stream wait
-    for every bucket, and hand the gradients to the optimizer (scaling / masking unless it does that itself)."""
-    if self.world > 1 and self._pending:
-      _, start, stop = self._buckets[-1]
-      if self._comm is not None:
-        for st in producer_streams:
-          self._comm.wait_stream(st)
-      self._all_reduce_slice(start, stop, None)
-      if self._comm is not None:
-        torch.cuda.current_stream(self.flat.device).wait_stream(self._comm)
-    self._pending = False
-    self.overlapped = False
-    self._post_reduce(model)
-
-  # -- blocking form ----------------------------------------------------------------
+  # -- exchange -------------------------------------------------------------------
   def reduce_gradients(self, model):
     """SUM the dense grads, AVERAGE everything the inner optimizer consumes (one all-reduce of the flat buffer)."""
     if self.world > 1:
@@ -149,8 +82,7 @@ class DataParallel(object):
     if self.world > 1 and not self.other_scale_in_optimizer:
       self.flat_other.mul_(1.0 / self.world)
     scale = 1.0 / self.world
-    layers = model.registry.layers() if model is not None else self._layers
-    for l in layers:
+    for l in model.registry.layers():
       g = l.masked_weights.dense_grad
       g.rigl_reduced = True
       if self.masked_grads_in_optimizer:

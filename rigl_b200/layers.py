@@ -112,9 +112,6 @@ WGRAD_SIDE_STREAM = False
 # mask * dense_grad while loading the dense gradient, so the layers neither compute nor return the masked
 # weight gradient (`weight.grad` stays untouched).
 MASKED_GRAD_IN_OPTIMIZER = False
-# data_parallel.DataParallel while a backward pass should launch its bucketed all-reduces (set by TrainHarness):
-# `layer_done(layer, stream)` is called right after a layer's dense wgrad has been issued on `stream`.
-DP_HOOK = None
 _WS_SLOT = ['main']
 _SIDE = {}
 _SIDE_KEEP = []        # tensors the side stream may still be reading (released at the join)
@@ -297,18 +294,12 @@ class _MaskedConvFn(torch.autograd.Function):
       finally:
         _WS_SLOT[0] = 'main'
       _SIDE_KEEP.append((x, dy16, patch_keep))     # no reuse of these blocks before the join
-      mw.fresh = True
-      mw.dense_grad.rigl_reduced = False           # rewritten: not yet summed over the replicas
-      if DP_HOOK is not None:
-        DP_HOOK.layer_done(layer, side)
     else:
       _timed('wgrad', layer, lambda: layer._wgrad(x, dy16, mw.dense_grad, accumulate=mw.fresh))
-      mw.fresh = True
-      mw.dense_grad.rigl_reduced = False
-      if DP_HOOK is not None:
-        DP_HOOK.layer_done(layer, None)
       if ctx.needs_input_grad[1] and not MASKED_GRAD_IN_OPTIMIZER:
         gw = layer.mask.apply_to(mw.dense_grad).view(layer.weight.shape)
+    mw.fresh = True
+    mw.dense_grad.rigl_reduced = False             # rewritten: not yet summed over the replicas
     gb = None
     if ctx.has_bias and ctx.needs_input_grad[2]:
       gb = dy.float().reshape(-1, layer.out_channels).sum(0) if dy.dim() == 2 else \

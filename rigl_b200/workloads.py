@@ -499,11 +499,6 @@ class TrainHarness(object):
     if pruning is not None:
       pruning.global_step = self.global_step
     self.dp = data_parallel
-    # Gradient exchange under data parallelism.  Default: ONE all-reduce of the flat buffer between the two graph
-    # replays (backward; optimizer).  RIGL_DP_OVERLAP=1: bucketed all-reduces launched from inside backward on a
-    # communication stream and captured with the step.  The exchange is short against a step and hiding it costs SM
-    # time beside the persistent one-CTA-per-SM conv kernels, so the simpler form is the default.
-    self._dp_overlap = os.environ.get('RIGL_DP_OVERLAP', '0') == '1'
     self._pack_ahead = on_cuda and os.environ.get('RIGL_PACK_AHEAD', '1') != '0'
     if self.dp is not None:
       self.dp.attach(model)
@@ -538,22 +533,14 @@ class TrainHarness(object):
     default from RIGL_WGRAD_OVERLAP (on unless '0')."""
     import os
     if overlap_wgrad is None:
-      # default on (RIGL_WGRAD_OVERLAP=0 keeps the serial backward); under data parallelism the bucketed
-      # all-reduces run behind the forked wgrad kernels on a third stream
+      # default on (RIGL_WGRAD_OVERLAP=0 keeps the serial backward)
       overlap_wgrad = os.environ.get('RIGL_WGRAD_OVERLAP', '1') != '0' 
     self._overlap = bool(overlap_wgrad)
     self._sx, self._sy = images.clone(), labels.clone()
-    ok = self._capture(warmup)
-    if not ok and self.dp is not None and self._dp_overlap:
-      # the collectives could not be captured on this stack: capture the step without them and all-reduce
-      # (blocking, one call) between the two replays instead of falling back to the eager step
-      self._dp_overlap = False
-      ok = self._capture(warmup)
-    return ok
+    return self._capture(warmup)
 
   def release_cuda_graph(self):
-    """Drops the captured graphs (back to the eager step).  Needed before torch.distributed is shut down: NCCL does
-    not finalise a communicator while graphs that captured its collectives exist."""
+    """Drops the captured graphs, so the memory their pool holds can be freed; later steps run eagerly."""
     self.graphed = False
     for name in ('_g_fb', '_g_opt', '_sloss'):
       if hasattr(self, name):
@@ -601,20 +588,11 @@ class TrainHarness(object):
     loss = F.cross_entropy(logits.float(), labels, label_smoothing=self.label_smoothing)
     layers.WGRAD_SIDE_STREAM = bool(getattr(self, '_overlap', False))
     layers.MASKED_GRAD_IN_OPTIMIZER = self.fused      # mask * dense_grad is formed inside the optimizer kernel
-    if self.dp is not None and self._dp_overlap:
-      self.dp.begin_backward()                        # bucketed all-reduces launched from inside backward
-      layers.DP_HOOK = self.dp
     try:
       loss.backward()
     finally:
       layers.WGRAD_SIDE_STREAM = False
       layers.MASKED_GRAD_IN_OPTIMIZER = False
-      layers.DP_HOOK = None
-      if self.dp is not None and self._dp_overlap:
-        # (only a side stream that was forked in THIS backward may be waited on: under capture a wait on a
-        #  stream outside the capture is an error)
-        side = list(layers._SIDE.values()) if getattr(self, '_overlap', False) else []
-        self.dp.finish(self.model, producer_streams=side)       # head bucket + join of the communication stream
       layers.join_side_streams()                # (no-op when nothing was forked)
     return loss
 
@@ -624,7 +602,7 @@ class TrainHarness(object):
     self._sy.copy_(labels, non_blocking=True)
     self._g_fb.replay()
     self.replayed_kernel_launches += self.graph_kernel_launches
-    if self.dp is not None and not self._dp_overlap:
+    if self.dp is not None:
       self.dp.reduce_gradients(self.model)
     gs = self.global_step
     def inner_step():
@@ -649,7 +627,7 @@ class TrainHarness(object):
     # without DP the grads are re-created by autograd (no zero-fill, no accumulate pass);
     # with DP they are views of the flat all-reduce buffer and must persist
     loss = self._forward_backward(images, labels, set_to_none=self.dp is None)
-    if self.dp is not None and not self._dp_overlap:
+    if self.dp is not None:
       self.dp.reduce_gradients(self.model)
     if self.opt is None:
       self.inner.step()

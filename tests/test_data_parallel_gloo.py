@@ -82,23 +82,16 @@ def _worker(rank, world, port):
   want = 3.0 * ref.registry.layers()[0].mask.dense / 2.0           # mask * dense / world
   assert torch.equal(l0.weight.grad, want)
   assert getattr(l0.masked_weights.dense_grad, 'rigl_reduced', False)
-  # the overlapped form: buckets of consecutive layers all-reduced as backward finishes them (last layer first),
-  # the head bucket (other gradients + first layers) in finish(); scaling folded into the optimizer
-  dp2 = DataParallel(bucket_elems=200).attach(model)
-  assert [b[0] for b in dp2._buckets] == [1, 0] and dp2._buckets[-1][1] == 0      # tail bucket, then the head
-  l0, l1 = model.registry.layers()
-  dp2.masked_grads_in_optimizer = dp2.other_scale_in_optimizer = True
+  # scaling folded into the fused optimizer: the exchange leaves SUMS and does not form the masked gradient
+  dp.masked_grads_in_optimizer = dp.other_scale_in_optimizer = True
   l0.masked_weights.dense_grad.fill_(rank + 1.0)
   l1.masked_weights.dense_grad.fill_(10.0 * (rank + 1))
   model.bias.grad.fill_(rank + 1.0)
+  l0.masked_weights.dense_grad.rigl_reduced = False
   w_grad_before = l0.weight.grad.clone()
-  dp2.begin_backward()
-  dp2.layer_done(l1)                                               # backward order: last layer first
-  assert torch.all(l1.masked_weights.dense_grad == 30.0)           # its bucket is already summed ...
-  assert torch.all(l0.masked_weights.dense_grad == rank + 1.0)     # ... the head bucket is not
-  dp2.layer_done(l0)
-  dp2.finish(model)
-  assert torch.all(l0.masked_weights.dense_grad == 3.0) and torch.all(model.bias.grad == 3.0)   # SUMS: 1/world is the optimizer's
+  dp.reduce_gradients(model)
+  assert torch.all(l0.masked_weights.dense_grad == 3.0) and torch.all(l1.masked_weights.dense_grad == 30.0)
+  assert torch.all(model.bias.grad == 3.0)                         # SUM: 1/world is the optimizer's
   assert torch.equal(l0.weight.grad, w_grad_before)               # masked gradient left to the fused optimizer
   assert getattr(l0.masked_weights.dense_grad, 'rigl_reduced', False)
   # diverging masks are detected
@@ -108,7 +101,7 @@ def _worker(rank, world, port):
   dist.destroy_process_group()
 
 
-def test_data_parallel_two_ranks_gloo():
+def test_data_parallel_one_all_reduce_two_ranks_gloo():
   with socket.socket() as s:
     s.bind(('127.0.0.1', 0))
     port = s.getsockname()[1]
