@@ -321,8 +321,8 @@ RIGL_API int rigl_im2col_nhwc(const rigl_conv_desc* d, const void* x, void* out,
  * ([N,(H+6)/2,(W+6)/2,16] bf16, rigl_stem_s2d_folded_bytes), the conv becomes a 4x4 stride-1 conv
  * whose 16 taps are fed from one shared-memory halo tile; rigl_stem_s2d_pack_weights writes the
  * [16 taps][cout][16] operand from the SAME HWIO weights + bitmap; _wgrad returns the dense
- * [7,7,cin,cout] gradient.  Requires ksize 7, stride 2, pad 3, cin <= 3, cout <= 64, even extents,
- * out_w <= 125. */
+ * [7,7,cin,cout] gradient.  Requires ksize 7, stride 2, pad 3, cin <= 3, cout a multiple of 8 up to 256
+ * (one grid row per 64 output channels), even extents, out_w <= 125. */
 RIGL_API int rigl_stem_s2d_supported(const rigl_conv_desc* d);
 RIGL_API size_t rigl_stem_s2d_folded_bytes(const rigl_conv_desc* d);
 RIGL_API size_t rigl_stem_s2d_packed_bytes(const rigl_conv_desc* d);

@@ -17,6 +17,11 @@
 // partials [th][tw*16 + k16][co] (rows 64..127 of each th block unused), then k_stem_s2d_reduce scatters them
 // into the dense HWIO gradient in CTA order (deterministic).
 //
+// Output channels come in groups of 64 (blockIdx.y): a CTA of group j holds the weight rows 64j .. 64j+63 and
+// writes / reads the output-gradient channels of that box; a ragged last group is zero-filled by the weight and
+// dY loads and clipped by the output store.  Every group runs the grid and strip order of a 64-channel launch, so
+// each group's output and gradient are those of a separate launch on its weight slice.
+//
 // Included by igemm_tc.cu inside namespace rigl.
 #pragma once
 
@@ -27,10 +32,11 @@ struct S2dParams {
   int R;                        // output rows per strip (= M tiles per strip)
   int nbuf;
   int strips_per_image, total_strips;
-  int N;                        // output channels (<= 64)
+  int N;                        // output channels (<= 256)
+  int groups;                   // 64-channel groups: gridDim.y
   uint32_t a_buf_bytes;         // halo tile incl. slack rows, multiple of 1024
   uint32_t a_tx_bytes;
-  float* wgrad_out;             // wgrad: [gridDim.x][4][128][64] fp32
+  float* wgrad_out;             // wgrad: [gridDim.x][groups][4][128][64] fp32
 };
 
 constexpr int kS2dWp = 128;                               // halo pitch (positions per M tile)
@@ -106,7 +112,7 @@ k_stem_s2d_fprop(const __grid_constant__ CUtensorMap amap, const __grid_constant
   if (warp == 0) {
     if (elect_one()) {
       mbar_arrive_expect_tx(b_full, 16 * kS2dBTapBytes);
-      for (int t = 0; t < 16; ++t) tma_load_3d(b_base + t * kS2dBTapBytes, &bmap, b_full, 0, 0, t);
+      for (int t = 0; t < 16; ++t) tma_load_3d(b_base + t * kS2dBTapBytes, &bmap, b_full, 0, 64 * blockIdx.y, t);
       int buf = 0; uint32_t phase = 0;
       for (int strip = blockIdx.x; strip < p.total_strips; strip += gridDim.x) {
         const int n = strip / p.strips_per_image, h0 = (strip % p.strips_per_image) * p.R;
@@ -157,7 +163,7 @@ k_stem_s2d_fprop(const __grid_constant__ CUtensorMap amap, const __grid_constant
         fence_proxy_async_smem();
         named_bar_sync(1, kConsumerThreads);
         if (issuer) {
-          tma_store_4d(&omap, slab, 0, 0, h0 + t, n);
+          tma_store_4d(&omap, slab, 64 * blockIdx.y, 0, h0 + t, n);
           tma_store_commit();
         }
         ++slab_ctr;
@@ -208,7 +214,7 @@ k_stem_s2d_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant
         mbar_arrive_expect_tx(full_bar(buf), p.a_tx_bytes + dy_bytes);
         const uint32_t x_dst = smem_base + buf * stage_bytes;
         tma_load_4d(x_dst, &xmap, full_bar(buf), 0, 0, h0, n);
-        tma_load_4d(x_dst + p.a_buf_bytes, &dymap, full_bar(buf), 0, 0, h0, n);
+        tma_load_4d(x_dst + p.a_buf_bytes, &dymap, full_bar(buf), 64 * blockIdx.y, 0, h0, n);
         if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
       }
     }
@@ -251,7 +257,7 @@ k_stem_s2d_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant
       if (lane == 0) mbar_arrive(empty_bar(buf));
       if (++buf == p.nbuf) { buf = 0; phase ^= 1u; }
     }
-    float* part = p.wgrad_out + (size_t)blockIdx.x * 4 * 128 * 64;
+    float* part = p.wgrad_out + ((size_t)blockIdx.x * p.groups + blockIdx.y) * 4 * 128 * 64;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int th = 2 * wg + i;
@@ -267,24 +273,26 @@ k_stem_s2d_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant
   }
 }
 
-// dw[kh][kw][c][co] = beta * dw + sum over CTAs of partial[cta][kh/2][(kw/2)*16 + ((kh&1)*2 + (kw&1))*3 + c][co]
+// dw[kh][kw][c][co] = beta * dw + sum over CTAs of partial[cta][co/64][kh/2][(kw/2)*16 + ((kh&1)*2 + (kw&1))*3 + c][co%64]
 __global__ void __launch_bounds__(256)
-k_stem_s2d_reduce(ConvGeom g, const float* __restrict__ part, int nparts, float* __restrict__ dw, float beta) {
+k_stem_s2d_reduce(ConvGeom g, const float* __restrict__ part, int nparts, int groups, float* __restrict__ dw,
+                  float beta) {
   const int total = g.ksize * g.ksize * g.cin * g.cout;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int co = i % g.cout, c = (i / g.cout) % g.cin, kw = (i / (g.cout * g.cin)) % g.ksize, kh = i / (g.cout * g.cin * g.ksize);
   const int th = kh >> 1, row = (kw >> 1) * 16 + ((kh & 1) * 2 + (kw & 1)) * 3 + c;
-  const float* src = part + ((size_t)th * 128 + row) * 64 + co;
+  const float* src = part + (((size_t)(co >> 6) * 4 + th) * 128 + row) * 64 + (co & 63);
+  const size_t cta_stride = (size_t)groups * 4 * 128 * 64;
   float a = beta != 0.f ? beta * dw[i] : 0.f;
-  for (int s = 0; s < nparts; ++s) a += src[(size_t)s * 4 * 128 * 64];
+  for (int s = 0; s < nparts; ++s) a += src[(size_t)s * cta_stride];
   dw[i] = a;
 }
 
 // ---------------------------------------------------------------------------- host side
 static bool s2d_geom(const ConvGeom& g, S2dParams* p, bool wgrad) {
   if (g.ksize != 7 || g.stride != 2 || g.pad != 3 || g.cin > 3 || g.cin < 1) return false;
-  if ((g.in_h & 1) || (g.in_w & 1) || g.cout > 64 || (g.cout % 8)) return false;
+  if ((g.in_h & 1) || (g.in_w & 1) || g.cout > 256 || (g.cout % 8)) return false;
   if (g.out_h != g.in_h / 2 || g.out_w != g.in_w / 2 || g.out_w + 3 > kS2dWp) return false;
   p->H = g.out_h; p->W = g.out_w; p->NB = g.batch;
   p->HS = (g.in_h + 2 * g.pad) / 2; p->WS = (g.in_w + 2 * g.pad) / 2;
@@ -294,6 +302,7 @@ static bool s2d_geom(const ConvGeom& g, S2dParams* p, bool wgrad) {
   p->strips_per_image = (g.out_h + p->R - 1) / p->R;
   p->total_strips = p->strips_per_image * g.batch;
   p->N = g.cout;
+  p->groups = (g.cout + 63) / 64;
   p->a_tx_bytes = (uint32_t)((p->R + 3) * kS2dWp) * 32u;
   p->a_buf_bytes = (uint32_t)(((size_t)((p->R + 3) * kS2dWp + 8) * 32 + 1023) / 1024 * 1024);
   p->wgrad_out = nullptr;
@@ -318,7 +327,7 @@ static int s2d_wgrad_grid(const S2dParams& p) {
 size_t s2d_workspace_bytes(const ConvGeom& g) {
   S2dParams p;
   if (!s2d_geom(g, &p, true)) return 0;
-  return (size_t)s2d_wgrad_grid(p) * 4 * 128 * 64 * sizeof(float) + 256;
+  return (size_t)s2d_wgrad_grid(p) * p.groups * 4 * 128 * 64 * sizeof(float) + 256;
 }
 
 int s2d_fold(const ConvGeom& g, const void* x, void* xs, cudaStream_t s) {
@@ -367,7 +376,7 @@ int s2d_fprop(const ConvGeom& g, const void* xs, const void* packed, void* y, cu
     configured = smem;
   }
   const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
-  const int grid = p.total_strips < sms ? p.total_strips : sms;
+  const dim3 grid(p.total_strips < sms ? p.total_strips : sms, p.groups);
   k_stem_s2d_fprop<<<grid, kThreads, smem, s>>>(amap, bmap, omap, p);
   RIGL_LAUNCH_CHECK("k_stem_s2d_fprop");
   return RIGL_OK;
@@ -380,7 +389,7 @@ int s2d_wgrad(const ConvGeom& g, const void* xs, const void* dy, float* dw, floa
   S2dParams p;
   if (!s2d_geom(g, &p, true)) { set_error("rigl_stem_s2d_wgrad: unsupported geometry"); return RIGL_ERR_UNSUPPORTED; }
   const int grid = s2d_wgrad_grid(p);
-  const size_t need = (size_t)grid * 4 * 128 * 64 * sizeof(float);
+  const size_t need = (size_t)grid * p.groups * 4 * 128 * 64 * sizeof(float);
   if (ws == nullptr || ws_bytes < need + 256) {
     set_error("rigl_stem_s2d_wgrad: workspace %zu < required %zu", ws_bytes, need + 256);
     return RIGL_ERR_WORKSPACE;
@@ -398,10 +407,10 @@ int s2d_wgrad(const ConvGeom& g, const void* xs, const void* dy, float* dw, floa
     RIGL_CUDA(cudaFuncSetAttribute(k_stem_s2d_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = smem;
   }
-  k_stem_s2d_wgrad<<<grid, kThreads, smem, s>>>(xmap, dymap, p);
+  k_stem_s2d_wgrad<<<dim3(grid, p.groups), kThreads, smem, s>>>(xmap, dymap, p);
   RIGL_LAUNCH_CHECK("k_stem_s2d_wgrad");
   const int total = g.ksize * g.ksize * g.cin * g.cout;
-  k_stem_s2d_reduce<<<(total + 255) / 256, 256, 0, s>>>(g, p.wgrad_out, grid, dw, beta);
+  k_stem_s2d_reduce<<<(total + 255) / 256, 256, 0, s>>>(g, p.wgrad_out, grid, p.groups, dw, beta);
   RIGL_LAUNCH_CHECK("k_stem_s2d_reduce");
   return RIGL_OK;
 }

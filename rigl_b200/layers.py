@@ -375,7 +375,7 @@ class SparseConv2d(_MaskedLayer):
       nbytes = int(_cabi.lib().rigl_packed_weights_bytes(1, self._kdim, self._cout))
       self.packed_patch = torch.zeros(nbytes, dtype=torch.uint8, device=device)
     self.s2d_mode = bool(STEM_S2D_PATH and self.patch_mode and k == 7 and s == 2 and int(in_channels) <= 3 and
-                         int(units) <= 64 and int(units) % 8 == 0 and padding == 'FIXED')
+                         int(units) <= 256 and int(units) % 8 == 0 and padding == 'FIXED')
     if self.s2d_mode:
       self.packed_s2d = torch.zeros(16 * int(units) * 32, dtype=torch.uint8, device=device)
     self._use_s2d = False

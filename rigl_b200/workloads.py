@@ -5,6 +5,7 @@ Only what BASELINE.json's configs need -- the shapes, variable names and wiring
 that the masked conv/linear kernels and the RigL update run on:
   ResNet50   rigl/imagenet_resnet/resnet_model.py:396-731 (v1.5: stride on the 3x3;
              BN after every conv, zero-init gamma on the last BN of a block)
+  ResNet     rigl/imagenet_resnet/resnet_model.py:577-805 (resnet_v1_: depths 18-200, width, prune flags)
   MnistFC    rigl/mnist/mnist_train_eval.py:112-160 (784-300-100-10, all masked)
   MobileNetV2 rigl/imagenet_resnet/mobilenetv2_model.py (inverted residual blocks, linear bottlenecks)
   VGG        rigl/imagenet_resnet/vgg.py (vgg_a / vgg_16 / vgg_19: 3x3 convs + ReLU, no BN; ReLU in the conv epilogues)
@@ -129,6 +130,130 @@ class ResNet50(nn.Module):
         x = blk(x, x_skip)
         x_skip = x
     x = x.mean(dim=(2, 3))
+    return self.final_dense(x)
+
+
+class _Residual(nn.Module):
+  """residual_block_ (resnet_model.py:306-403), the basic block of ResNet-18 / 34: two 3x3 convs, the first one
+  strided, BN after each; the last BN has zero-init gamma and takes the residual add + final ReLU, in the form of
+  _Bottleneck.bn3."""
+
+  def __init__(self, cin, filters, strides, use_projection, name, device, registry):
+    super(_Residual, self).__init__()
+    mk = lambda ci, co, k, s, n: SparseConv2d(ci, co, k, strides=s, padding='FIXED', name='resnet_model/' + n,
+                                              device=device, registry=registry)
+    self.proj = None
+    if use_projection:
+      self.proj = mk(cin, filters, 1, strides, 'residual_projection_%s' % name)
+      self.proj_bn = _BNReLU(filters, relu=False, device=device)
+    self.conv1 = mk(cin, filters, 3, strides, 'residual_1_%s' % name)
+    self.bn1 = _BNReLU(filters, device=device)
+    self.conv2 = mk(filters, filters, 3, 1, 'residual_2_%s' % name)
+    for conv in (self.proj, self.conv1, self.conv2):
+      if conv is not None:
+        conv.collect_bn_stats = True
+    self.bn2 = _BNReLU(filters, relu=True, init_zero=True, device=device)
+
+  def forward(self, x, x_skip=None, fork=False):
+    """As _Bottleneck.forward: `x_skip` is the shortcut's handle of the input, `fork` returns two handles."""
+    if x_skip is None:
+      x_skip = x
+    shortcut = x_skip if self.proj is None else conv_bn(self.proj, self.proj_bn, x_skip)
+    y = conv_bn(self.conv1, self.bn1, x)
+    return conv_bn(self.conv2, self.bn2, y, residual=shortcut, fork=fork)   # relu(BN(conv2) + shortcut)
+
+
+# resnet_depth -> (block, blocks per group), resnet_model.py:777-802
+RESNET_DEPTHS = {18: ('residual', (2, 2, 2, 2)), 34: ('residual', (3, 4, 6, 3)), 50: ('bottleneck', (3, 4, 6, 3)),
+                 101: ('bottleneck', (3, 4, 23, 3)), 152: ('bottleneck', (3, 8, 36, 3)),
+                 200: ('bottleneck', (3, 24, 36, 3))}
+
+
+def resnet_plan(depth, width=1.0):
+  """Channel plan of resnet_v1_(depth, width): (block kind 'residual' or 'bottleneck', initial_conv filters,
+  [(block name, cin, filters, stride, projection)], final_dense inputs).  Block names are block_group's: the first
+  block of group g is 'block_group_projection_block_group<g>' (projection shortcut, the group's stride -- group 1
+  included, at stride 1), block b > 0 'block_group<g>_<b>_1'.  A bottleneck block's output has 4 * filters channels.
+  Every width must be a multiple of 8 (the NHWC kernels move 8 channels per 16-byte vector); ValueError names the
+  first layer that is not."""
+  if depth not in RESNET_DEPTHS:
+    raise ValueError('Not a valid resnet_depth: %r (one of %s)' % (depth, sorted(RESNET_DEPTHS)))
+  kind, counts = RESNET_DEPTHS[depth]
+  mult = 4 if kind == 'bottleneck' else 1
+  prefix = 'bottleneck' if kind == 'bottleneck' else 'residual'
+
+  def need8(c, layer):
+    if c % 8:
+      raise ValueError('ResNet(%d, width=%g): %s has %d channels, not a multiple of 8' % (depth, width, layer, c))
+  c0 = int(64 * width)
+  need8(c0, 'resnet_model/initial_conv')
+  blocks, cin = [], c0
+  for g, (base, n_blocks, stride) in enumerate(zip((64, 128, 256, 512), counts, (1, 2, 2, 2)), 1):
+    filters = int(base * width)
+    for b in range(n_blocks):
+      name = 'block_group_projection_block_group%d' % g if b == 0 else 'block_group%d_%d_1' % (g, b)
+      if b == 0:
+        need8(mult * filters, 'resnet_model/%s_projection_%s' % (prefix, name))
+      need8(filters, 'resnet_model/%s_1_%s' % (prefix, name))
+      blocks.append((name, cin, filters, stride if b == 0 else 1, b == 0))
+      cin = mult * filters
+  return kind, c0, blocks, cin
+
+
+class ResNet(nn.Module):
+  """resnet_v1_(depth, num_classes, width, prune_first_layer, prune_last_layer) (resnet_model.py:577-805): ResNet-18
+  / 34 on the basic block (_Residual), ResNet-50 / 101 / 152 / 200 on the bottleneck (_Bottleneck), every width
+  int(c * width).  ResNet(50) builds ResNet50's scopes, shapes and modules in the same order, so it draws the same
+  initial weights under one seed.  With prune_first_layer=False the 7x7/2 `initial_conv` is a dense conv, with
+  prune_last_layer=False `final_dense` a dense fp32 layer with a zero bias; neither is masked, both keep the l2
+  regularizer (evaluate.regularized_kernels), as in the reference."""
+
+  def __init__(self, depth, num_classes=1000, width=1.0, prune_first_layer=True, prune_last_layer=True,
+               device='cuda', registry=None):
+    super(ResNet, self).__init__()
+    kind, c0, plan, fc_in = resnet_plan(depth, width)     # (raises before any parameter exists)
+    self.depth, self.width = depth, width
+    self.registry = registry if registry is not None else pruning.MaskedLayerRegistry()
+    reg = self.registry
+    self.prune_first_layer = bool(prune_first_layer)
+    if self.prune_first_layer:
+      self.initial_conv = SparseConv2d(3, c0, 7, strides=2, padding='FIXED', name='resnet_model/initial_conv',
+                                       device=device, registry=reg)
+      self.initial_conv.collect_bn_stats = True
+    else:             # conv2d_fixed_padding with pruning_method 'baseline': not masked
+      self.initial_conv = DenseConv2d(3, c0, 7, stride=2, padding=3, bias=False, device=device)
+      variance_scaling_(self.initial_conv.weight.data.permute(2, 3, 1, 0))
+    self.initial_bn = _BNReLU(c0, device=device)
+    block = _Bottleneck if kind == 'bottleneck' else _Residual
+    self.blocks = nn.ModuleList([block(cin, filters, stride, proj, name, device, reg)
+                                 for name, cin, filters, stride, proj in plan])
+    self.prune_last_layer = bool(prune_last_layer)
+    if self.prune_last_layer:
+      self.final_dense = SparseLinear(fc_in, num_classes, name='resnet_model/final_dense', device=device,
+                                      registry=reg, out_dtype=torch.float32,
+                                      kernel_initializer=lambda w: w.normal_(0., .01))
+    else:             # sparse_fully_connected with sparsity_technique 'baseline' (tf.layers.dense): fp32, zero bias
+      self.final_dense = nn.Linear(fc_in, num_classes, device=device)
+      with torch.no_grad():
+        self.final_dense.weight.normal_(0., .01)
+        self.final_dense.bias.zero_()
+
+  def forward(self, x):
+    if self.prune_first_layer:
+      x = conv_bn(self.initial_conv, self.initial_bn, x)
+    else:
+      x = self.initial_bn(self.initial_conv(x.to(torch.bfloat16).contiguous(memory_format=torch.channels_last)))
+    x = max_pool_same(x, 3, 2)
+    x_skip, last = x, len(self.blocks) - 1
+    for i, blk in enumerate(self.blocks):
+      if i < last and FORK_BLOCK_OUTPUTS:
+        x, x_skip = blk(x, x_skip, fork=True)
+      else:
+        x = blk(x, x_skip)
+        x_skip = x
+    x = x.mean(dim=(2, 3))
+    if not self.prune_last_layer:
+      x = x.float()
     return self.final_dense(x)
 
 
