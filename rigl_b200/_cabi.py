@@ -50,6 +50,9 @@ class ConvDesc(C.Structure):
               ('ksize', C.c_int32), ('stride', C.c_int32), ('pad', C.c_int32), ('x_pitch', C.c_int32)]
 
 
+# rigl_status: a fused conv entry point returns it, with nothing launched, where the layer's kernel has no such epilogue
+RIGL_ERR_UNSUPPORTED = -4
+
 GROW_ZEROS, GROW_TENSOR, GROW_GRAD_SCALE, GROW_GRAD_SIGN = 0, 1, 2, 3
 LAYER_GROW_SCORE_SIGNED, LAYER_DROP_ONLY, LAYER_ALL_ACTIVE = 1, 2, 4
 

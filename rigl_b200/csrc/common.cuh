@@ -22,10 +22,10 @@ inline int cuda_fail(cudaError_t e, const char* what) {
   return RIGL_ERR_CUDA;
 }
 
-#define RIGL_CUDA(expr)                                        \
-  do {                                                         \
-    cudaError_t _e = (expr);                                   \
-    if (_e != cudaSuccess) return ::rigl::cuda_fail(_e, #expr); \
+#define RIGL_CUDA(...)                                                \
+  do {                                                                \
+    cudaError_t _e = (__VA_ARGS__);                                   \
+    if (_e != cudaSuccess) return ::rigl::cuda_fail(_e, #__VA_ARGS__); \
   } while (0)
 
 #define RIGL_LAUNCH_CHECK(name)                                 \

@@ -1,6 +1,5 @@
-// C-ABI entry points of the masked conv / linear path: argument validation and
-// the shape dispatch between the wgmma implicit-GEMM kernels (igemm_tc.cu)
-// and the CUDA-core kernels (conv_simt.cu).
+// C-ABI entry points of the masked conv / linear path: argument validation, then conv_route (igemm_tc.cu) picks
+// the wgmma implicit-GEMM or halo kernels (igemm_tc.cu) or the CUDA-core kernels (conv_simt.cu).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -10,7 +9,7 @@ namespace rigl {
 
 static int g_force_simt = -1;
 
-static bool force_simt() {
+bool force_simt() {
   if (g_force_simt < 0) {
     const char* e = getenv("RIGL_FORCE_SIMT");
     g_force_simt = (e && e[0] == '1') ? 1 : 0;
@@ -113,6 +112,28 @@ extern "C" size_t rigl_conv_workspace_bytes(const rigl_conv_desc* d) {
   return tc_workspace_bytes(g);
 }
 
+// Routes one fprop / dgrad and runs it.  The CUDA-core fprop reads the dgrad-layout weights of the packed blob, the
+// CUDA-core dgrad the fprop-layout ones.
+static int run_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, const ConvEpilogue& epi,
+                     void* stream) {
+  const int path = conv_route(g, 0, epi);
+  if (path < 0) return path;
+  if (path == kPathSimt)
+    return simt_fprop(g, x, static_cast<const uint8_t*>(packed) + packed_layout(g.taps(), g.cin, g.cout).off_dgrad, y,
+                      epi.out_f32, epi.bias, (cudaStream_t)stream);
+  return tc_fprop(g, path, x, packed, y, epi, (cudaStream_t)stream);
+}
+
+static int run_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, const ConvEpilogue& epi,
+                     void* stream) {
+  const int path = conv_route(g, 1, epi);
+  if (path < 0) return path;
+  if (path == kPathSimt)
+    return simt_dgrad(g, dy, static_cast<const uint8_t*>(packed) + packed_layout(g.taps(), g.cin, g.cout).off_fprop,
+                      dx, (cudaStream_t)stream);
+  return tc_dgrad(g, path, dy, packed, dx, epi, (cudaStream_t)stream);
+}
+
 extern "C" int rigl_masked_conv2d_fprop(const rigl_conv_desc* d, const void* x, const void* packed,
                                         void* y_bf16, float* y_f32, const float* bias, void* ws,
                                         size_t ws_bytes, void* stream) {
@@ -120,11 +141,9 @@ extern "C" int rigl_masked_conv2d_fprop(const rigl_conv_desc* d, const void* x, 
   int rc = geom_from_desc(d, &g);
   if (rc != RIGL_OK) return rc;
   RIGL_REQUIRE(x && packed && (y_bf16 || y_f32), "rigl_masked_conv2d_fprop: null tensor");
-  const PackedLayout L = packed_layout(g.taps(), g.cin, g.cout);
-  if (!force_simt() && tc_supported(g, 0))
-    return tc_fprop(g, x, packed, y_bf16, y_f32, bias, ws, ws_bytes, (cudaStream_t)stream);
-  return simt_fprop(g, x, static_cast<const uint8_t*>(packed) + L.off_dgrad, y_bf16, y_f32, bias,
-                    (cudaStream_t)stream);
+  ConvEpilogue epi;
+  epi.out_f32 = y_f32; epi.bias = bias;
+  return run_fprop(g, x, packed, y_bf16, epi, stream);
 }
 
 extern "C" int rigl_bn_partial_rows(void) { return tc_max_ctas(); }
@@ -141,11 +160,10 @@ extern "C" int rigl_masked_conv2d_fprop_bnstats(const rigl_conv_desc* d, const v
   int rc = geom_from_desc(d, &g);
   if (rc != RIGL_OK) return rc;
   RIGL_REQUIRE(x && packed && y_bf16 && bn_partial && bn_rows_out, "rigl_masked_conv2d_fprop_bnstats: null argument");
-  if (force_simt() || !tc_supported(g, 0)) {
-    set_error("rigl_masked_conv2d_fprop_bnstats: shape not on the tensor-core path");
-    return RIGL_ERR_UNSUPPORTED;
-  }
-  return tc_fprop(g, x, packed, y_bf16, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream, bn_partial, bn_rows_out);
+  ConvEpilogue epi;
+  epi.kind = ConvEpilogue::kBnStats;
+  epi.bn_partial = bn_partial; epi.bn_rows = bn_rows_out;
+  return run_fprop(g, x, packed, y_bf16, epi, stream);
 }
 
 extern "C" int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const void* x, const void* packed,
@@ -158,12 +176,10 @@ extern "C" int rigl_masked_conv2d_fprop_bnapply(const rigl_conv_desc* d, const v
   RIGL_REQUIRE(g.cout % 8 == 0, "rigl_masked_conv2d_fprop_bnapply: cout %d is not a multiple of 8", g.cout);
   RIGL_REQUIRE(aligned16(x) && aligned16(y_bf16) && aligned16(residual),
                "rigl_masked_conv2d_fprop_bnapply: tensors must be 16-byte aligned");
-  if (force_simt() || !tc_supported(g, 0)) {    // (this includes the 3-channel stem)
-    set_error("rigl_masked_conv2d_fprop_bnapply: shape not on the K-major tensor-core kernel");
-    return RIGL_ERR_UNSUPPORTED;
-  }
-  const BnApplyArgs bn = {residual, scale, shift, relu};
-  return tc_fprop(g, x, packed, y_bf16, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream, nullptr, nullptr, &bn);
+  ConvEpilogue epi;
+  epi.kind = ConvEpilogue::kBnApply;
+  epi.residual = residual; epi.scale = scale; epi.shift = shift; epi.relu = relu;
+  return run_fprop(g, x, packed, y_bf16, epi, stream);
 }
 
 extern "C" int rigl_masked_conv2d_fprop_relu(const rigl_conv_desc* d, const void* x, const void* packed, void* y_bf16,
@@ -174,12 +190,9 @@ extern "C" int rigl_masked_conv2d_fprop_relu(const rigl_conv_desc* d, const void
   RIGL_REQUIRE(x && packed && y_bf16, "rigl_masked_conv2d_fprop_relu: null argument");
   RIGL_REQUIRE(g.cout % 8 == 0, "rigl_masked_conv2d_fprop_relu: cout %d is not a multiple of 8", g.cout);
   RIGL_REQUIRE(aligned16(x) && aligned16(y_bf16), "rigl_masked_conv2d_fprop_relu: tensors must be 16-byte aligned");
-  if (force_simt() || !tc_supported(g, 0)) {
-    set_error("rigl_masked_conv2d_fprop_relu: shape not on the tensor-core kernels");
-    return RIGL_ERR_UNSUPPORTED;
-  }
-  return tc_fprop(g, x, packed, y_bf16, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream, nullptr, nullptr,
-                  nullptr, true);
+  ConvEpilogue epi;
+  epi.kind = ConvEpilogue::kRelu;
+  return run_fprop(g, x, packed, y_bf16, epi, stream);
 }
 
 extern "C" int rigl_masked_conv2d_dgrad_relu(const rigl_conv_desc* d, const void* dy, const void* packed,
@@ -193,11 +206,10 @@ extern "C" int rigl_masked_conv2d_dgrad_relu(const rigl_conv_desc* d, const void
                g.x_pitch);
   RIGL_REQUIRE(aligned16(dy) && aligned16(x) && aligned16(dx),
                "rigl_masked_conv2d_dgrad_relu: tensors must be 16-byte aligned");
-  if (force_simt() || !tc_supported(g, 1) || g.stride != 1) {
-    set_error("rigl_masked_conv2d_dgrad_relu: shape has no gated dgrad (stride %d)", g.stride);
-    return RIGL_ERR_UNSUPPORTED;
-  }
-  return tc_dgrad(g, dy, packed, dx, ws, ws_bytes, (cudaStream_t)stream, x);
+  ConvEpilogue epi;
+  epi.kind = ConvEpilogue::kReluGate;
+  epi.gate = x;
+  return run_dgrad(g, dy, packed, dx, epi, stream);
 }
 
 extern "C" int rigl_masked_conv2d_dgrad(const rigl_conv_desc* d, const void* dy, const void* packed,
@@ -206,10 +218,7 @@ extern "C" int rigl_masked_conv2d_dgrad(const rigl_conv_desc* d, const void* dy,
   int rc = geom_from_desc(d, &g);
   if (rc != RIGL_OK) return rc;
   RIGL_REQUIRE(dy && packed && dx, "rigl_masked_conv2d_dgrad: null tensor");
-  const PackedLayout L = packed_layout(g.taps(), g.cin, g.cout);
-  if (!force_simt() && tc_supported(g, 1))
-    return tc_dgrad(g, dy, packed, dx, ws, ws_bytes, (cudaStream_t)stream);
-  return simt_dgrad(g, dy, static_cast<const uint8_t*>(packed) + L.off_fprop, dx, (cudaStream_t)stream);
+  return run_dgrad(g, dy, packed, dx, ConvEpilogue(), stream);
 }
 
 extern "C" int rigl_conv2d_wgrad_dense(const rigl_conv_desc* d, const void* x, const void* dy, float* dw,
@@ -219,7 +228,7 @@ extern "C" int rigl_conv2d_wgrad_dense(const rigl_conv_desc* d, const void* x, c
   if (rc != RIGL_OK) return rc;
   RIGL_REQUIRE(x && dy && dw, "rigl_conv2d_wgrad_dense: null tensor");
   RIGL_REQUIRE(beta == 0.f || beta == 1.f, "rigl_conv2d_wgrad_dense: beta must be 0 or 1");
-  if (!force_simt() && tc_supported(g, 2))
-    return tc_wgrad(g, x, dy, dw, beta, ws, ws_bytes, (cudaStream_t)stream);
-  return simt_wgrad(g, x, dy, dw, beta, (cudaStream_t)stream);
+  const int path = conv_route(g, 2, ConvEpilogue());
+  if (path == kPathSimt) return simt_wgrad(g, x, dy, dw, beta, (cudaStream_t)stream);
+  return tc_wgrad(g, path, x, dy, dw, beta, ws, ws_bytes, (cudaStream_t)stream);
 }

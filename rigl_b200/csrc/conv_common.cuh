@@ -51,30 +51,48 @@ int simt_dgrad(const ConvGeom& g, const void* dy, const void* w_fprop, void* dx,
 int simt_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float beta, cudaStream_t s);
 int simt_im2col(const ConvGeom& g, const void* x, void* out, int64_t out_pitch, cudaStream_t s);
 
-// Inference batch norm applied by the K-major fprop epilogue (rigl_masked_conv2d_fprop_bnapply):
-// y = [relu](conv * scale + shift [+ residual]), residual bf16 in y's layout or null.
-struct BnApplyArgs {
-  const void* residual;
-  const float* scale;
-  const float* shift;
-  int relu;
+// What a conv pass does with its result D besides storing it as bf16: the kind, and the pointers that kind uses.
+struct ConvEpilogue {
+  enum Kind { kPlain, kBnStats, kBnApply, kRelu, kReluGate };
+  Kind kind = kPlain;
+  // kPlain fprop: fp32 output and/or bias, stored straight from the registers (the dense layer)
+  float* out_f32 = nullptr;
+  const float* bias = nullptr;
+  // kBnStats (fprop): bn_partial[rows][2][cout] receives per-CTA column sums / sums of squares of the stored output,
+  // *bn_rows the number of rows
+  float* bn_partial = nullptr;
+  int* bn_rows = nullptr;
+  // kBnApply (fprop): y = [relu](conv * scale + shift [+ residual]), residual bf16 in y's layout or null
+  const void* residual = nullptr;
+  const float* scale = nullptr;
+  const float* shift = nullptr;
+  int relu = 0;
+  // kRelu (fprop): y = bf16(relu(conv)).  kReluGate (dgrad): dx = gate > 0 ? conv^T(dy) : 0, gate bf16 in dx's layout
+  const void* gate = nullptr;
 };
 
-// tensor-core path (igemm_tc.cu)
+// Kernels that run a conv pass: the CUDA-core kernels (conv_simt.cu), the halo kernels (halo3x3.cuh) or the
+// K-major / wgrad implicit-GEMM kernels (igemm_tc.cu).  Positive, so conv_route can return them or a RIGL_ERR_*.
+enum ConvPath { kPathSimt = 1, kPathHalo = 2, kPathKmajor = 3 };
+
+// The one place that decides which kernels run pass `which` (0 fprop, 1 dgrad, 2 wgrad) of layer g with epilogue epi.
+// Returns a ConvPath, or RIGL_ERR_UNSUPPORTED with the last error set when no kernel has that epilogue for g:
+// the CUDA-core path (RIGL_FORCE_SIMT=1 or a shape the tensor-core kernels cannot address) has only kPlain; the halo
+// kernels only kPlain and kRelu; kReluGate needs stride 1; kBnStats needs a reduction long enough to hide the
+// statistics (taps * cin >= 512, or >= 256 with cout <= 128) unless tc_set_bn_stats_always.  No CUDA call.
+int conv_route(const ConvGeom& g, int which, const ConvEpilogue& epi);
+bool force_simt();   // RIGL_FORCE_SIMT=1 / rigl_set_force_simt(1): every conv pass on the CUDA-core kernels
+
+// tensor-core path (igemm_tc.cu): `path` is conv_route's kPathHalo or kPathKmajor for the same arguments.
 bool tc_supported(const ConvGeom& g, int which /*0 fprop, 1 dgrad, 2 wgrad*/);
 size_t tc_workspace_bytes(const ConvGeom& g);
-// bn_apply != null: RIGL_ERR_UNSUPPORTED unless the layer runs on k_igemm_kmajor with the TMA-store epilogue.
-// relu: y = bf16(relu(conv)) from the K-major or halo epilogue.
-int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32,
-             const float* bias, void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial = nullptr,
-             int* bn_rows = nullptr, const BnApplyArgs* bn_apply = nullptr, bool relu = false);
+int tc_fprop(const ConvGeom& g, int path, const void* x, const void* packed, void* y, const ConvEpilogue& epi,
+             cudaStream_t s);
 int tc_max_ctas();
 void tc_set_bn_stats_always(bool on);
-// gate != null (bf16 in dx's layout and pitch): dx = gate > 0 ? conv^T(dy) : 0 from the K-major epilogue; the halo
-// dgrad and stride > 1 return RIGL_ERR_UNSUPPORTED before any launch.
-int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, void* ws,
-             size_t ws_bytes, cudaStream_t s, const void* gate = nullptr);
-int tc_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float beta, void* ws,
+int tc_dgrad(const ConvGeom& g, int path, const void* dy, const void* packed, void* dx, const ConvEpilogue& epi,
+             cudaStream_t s);
+int tc_wgrad(const ConvGeom& g, int path, const void* x, const void* dy, float* dw, float beta, void* ws,
              size_t ws_bytes, cudaStream_t s);
 
 // space-to-depth 7x7/2 stem (stem_s2d.cuh, included by igemm_tc.cu)

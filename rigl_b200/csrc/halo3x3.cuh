@@ -280,7 +280,7 @@ k_halo3x3_wgrad(const __grid_constant__ CUtensorMap xmap, const __grid_constant_
 
 // Geometry the halo kernels cover; `kred` = reduction channels per tap (cin for fprop, cout for dgrad).
 static bool halo_geom(const ConvGeom& g, int kred, HaloParams* p, size_t smem_fixed, int dy_tile) {
-  if (!g_halo || g.ksize != 3 || g.stride != 1 || g.pad != 1) return false;
+  if (!halo_enabled() || g.ksize != 3 || g.stride != 1 || g.pad != 1) return false;
   if (g.in_h != g.out_h || g.in_w != g.out_w || kred > 64 || kred % 8) return false;
   int wp = 8;
   while (wp < g.in_w + 2) wp *= 2;
@@ -356,12 +356,8 @@ static int halo_launch_kmajor(HaloParams p, const void* in, int kred, int in_pit
   rc = make_act_map(&omap, out, p.NB, p.H, p.W, n_out, out_pitch, 1, 0, 0, obox);
   if (rc != RIGL_OK) return rc;
   const size_t smem = 9 * kHaloBTapBytes + p.nbuf * (size_t)p.a_buf_bytes + 2 * kHaloSlabBytes + 1024 + 256;
-  static size_t configured[2] = {0, 0};
+  RIGL_CUDA(relu ? smem_limit<k_halo3x3_kmajor_relu>(smem) : smem_limit<k_halo3x3_kmajor>(smem));
   auto kern = relu ? k_halo3x3_kmajor_relu : k_halo3x3_kmajor;
-  if (smem > configured[relu]) {
-    RIGL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured[relu] = smem;
-  }
   const int n_tiles = (n_out + 63) / 64;
   const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   int gx = sms / n_tiles;
@@ -387,11 +383,7 @@ static int halo_launch_wgrad(HaloParams p, const ConvGeom& g, const void* x, con
   rc = make_act_map(&dymap, dy, p.NB, p.H, p.W, g.cout, g.cout, 1, 0, 0, dbox);
   if (rc != RIGL_OK) return rc;
   const size_t smem = p.nbuf * ((size_t)p.a_buf_bytes + (size_t)p.R * p.Wp * 128) + 1024 + 256;
-  static size_t configured = 0;
-  if (smem > configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_halo3x3_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
+  RIGL_CUDA(smem_limit<k_halo3x3_wgrad>(smem));
   k_halo3x3_wgrad<<<(unsigned)halo_wgrad_grid(p), kHaloWgradThreads, smem, s>>>(xmap, dymap, p);
   RIGL_LAUNCH_CHECK("k_halo3x3_wgrad");
   return RIGL_OK;

@@ -658,7 +658,6 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 
 static EncodeTiledFn g_encode = nullptr;
 static bool g_bn_stats_always = false;   // rigl_set_bn_stats_always: epilogue statistics for every supported shape (tests)
-static bool g_halo = true;          // RIGL_HALO3X3=0: 3x3/s1 layers with <= 64 channels use the generic kernels
 static int g_num_sms = 0;
 static std::once_flag g_once;
 static int g_init_status = RIGL_OK;
@@ -673,7 +672,6 @@ static void init_driver() {
     return;
   }
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  if (const char* e = getenv("RIGL_HALO3X3")) g_halo = !(e[0] == '0');
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
@@ -690,6 +688,26 @@ static int ensure_driver() {
   }
   std::call_once(g_once, init_driver);
   return g_init_status;
+}
+
+// RIGL_HALO3X3=0: 3x3/s1 layers with <= 64 channels use the generic kernels.
+static bool halo_enabled() {
+  static const bool on = [] {
+    const char* e = getenv("RIGL_HALO3X3");
+    return !(e && e[0] == '0');
+  }();
+  return on;
+}
+
+// Raises kernel K's dynamic shared-memory limit to `smem` bytes the first time a launch needs that much.  The limit
+// only grows, so a smaller launch after a larger one makes no call.
+template <auto K>
+static cudaError_t smem_limit(size_t smem) {
+  static size_t configured = 0;
+  if (smem <= configured) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e == cudaSuccess) configured = smem;
+  return e;
 }
 
 // bf16 tensor map over `rank` dims (dim 0 innermost, contiguous), 128B swizzle, zero OOB fill.
@@ -820,66 +838,91 @@ size_t tc_workspace_bytes(const ConvGeom& g) {
   return elems * sizeof(float) + 256;
 }
 
+int conv_route(const ConvGeom& g, int which, const ConvEpilogue& epi) {
+  static const char* const kName[] = {"plain", "fused BN statistics", "fused BN apply", "fused ReLU", "gated dgrad"};
+  const char* name = kName[epi.kind];
+  if (force_simt() || !tc_supported(g, which)) {
+    if (epi.kind == ConvEpilogue::kPlain) return kPathSimt;
+    set_error("%s: shape not on the tensor-core kernels", name);
+    return RIGL_ERR_UNSUPPORTED;
+  }
+  if (epi.kind == ConvEpilogue::kReluGate && g.stride != 1) {   // the strided dgrad is one launch per parity class
+    set_error("%s: shape has no gated dgrad (stride %d)", name, g.stride);
+    return RIGL_ERR_UNSUPPORTED;
+  }
+  HaloParams hp;
+  const bool halo = which == 0   ? epi.out_f32 == nullptr && epi.bias == nullptr && halo_fprop_ok(g, &hp)
+                    : which == 1 ? halo_dgrad_ok(g, &hp)
+                                 : halo_wgrad_ok(g, &hp);
+  if (halo) {
+    if (epi.kind == ConvEpilogue::kPlain || epi.kind == ConvEpilogue::kRelu) return kPathHalo;
+    set_error("%s: layer runs on the halo kernels", name);   // the caller runs the plain call + the separate pass
+    return RIGL_ERR_UNSUPPORTED;
+  }
+  if (epi.kind == ConvEpilogue::kBnStats && !g_bn_stats_always) {
+    // The statistics are free when the tile's main loop is long enough to hide them (reduction length
+    // K = taps * cin >= 512), and cost about what the separate stats pass costs -- or more -- for the short-K /
+    // wide-output layers whose epilogue is the bottleneck (1x1 convs with K <= 128; K = 256 with more than 128
+    // output channels).
+    const int K = g.taps() * g.cin;
+    if (!(K >= 512 || (K >= 256 && g.cout <= 128))) {
+      set_error("%s: not profitable for this shape (K = %d, cout = %d)", name, K, g.cout);
+      return RIGL_ERR_UNSUPPORTED;
+    }
+  }
+  return kPathKmajor;
+}
+
 static int kmajor_grid(const IgemmParams& p) {         // CTAs the K-major launcher will use (p.n_tiles set)
   const int tiles = p.tiles_w * p.tiles_h * p.tiles_n * p.n_tiles;
   return tiles < g_num_sms ? tiles : g_num_sms;
 }
 
-// The ReLU epilogues of k_igemm_kmajor_relu (launch_kmajor's `relu`).
-enum ReluEpi { kReluNone = 0, kReluFprop = 1, kReluGateDgrad = 2 };
-
-template <int BN, int STAGES, bool kGate>
-static int launch_kmajor_relu(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
-                              const IgemmParams& p, cudaStream_t s, const CUtensorMap& rmap, size_t smem) {
-  static bool configured = false;
-  if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_relu<BN, STAGES, kGate>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
-  k_igemm_kmajor_relu<BN, STAGES, kGate><<<kmajor_grid(p), kThreads, smem, s>>>(amaps, bmap, omap, p, rmap);
-  RIGL_LAUNCH_CHECK("k_igemm_kmajor_relu");
-  return RIGL_OK;
-}
-
-// ep != null: the batch-norm epilogue variant (k_igemm_kmajor_bn) with the residual map *rmap.  relu != kReluNone:
-// the ReLU variant (k_igemm_kmajor_relu), with the gate map *rmap for kReluGateDgrad.
+// The K-major kernel with epi's epilogue: k_igemm_kmajor (kPlain; kBnStats through p.bn_partial), k_igemm_kmajor_bn
+// (kBnApply, residual map rmap) or k_igemm_kmajor_relu (kRelu; kReluGate with the gate map rmap).  Variants that read
+// no second tensor get the output map as rmap.
 template <int BN, int STAGES>
 static int launch_kmajor(const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap, const IgemmParams& p,
-                         cudaStream_t s, const CUtensorMap* rmap, const BnEpilogue* ep, int relu) {
+                         const ConvEpilogue& epi, const CUtensorMap& rmap, cudaStream_t s) {
   // (the 256 bytes past the slabs hold the 2 * STAGES ring barriers and the residual barrier)
   constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 2 * (kBM * 64 * 2) + 1024 + 256;
   static_assert(smem <= 227 * 1024, "K-major kernel exceeds the shared memory of an SM");
   static_assert(8 * (2 * STAGES + 1) <= 256, "K-major kernel barriers exceed their shared memory");
-  if (relu == kReluFprop) return launch_kmajor_relu<BN, STAGES, false>(amaps, bmap, omap, p, s, omap, smem);
-  if (relu == kReluGateDgrad) return launch_kmajor_relu<BN, STAGES, true>(amaps, bmap, omap, p, s, *rmap, smem);
-  if (ep != nullptr) {
-    static bool configured_bn = false;
-    if (!configured_bn) {
-      RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor_bn<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem));
-      configured_bn = true;
+  const int grid = kmajor_grid(p);
+  const char* name;
+  switch (epi.kind) {
+    case ConvEpilogue::kBnApply: {
+      const BnEpilogue ep = {epi.scale, epi.shift, epi.relu ? 1 : 0, epi.residual ? 1 : 0};
+      RIGL_CUDA(smem_limit<k_igemm_kmajor_bn<BN, STAGES>>(smem));
+      k_igemm_kmajor_bn<BN, STAGES><<<grid, kThreads, smem, s>>>(amaps, bmap, omap, p, rmap, ep);
+      name = "k_igemm_kmajor_bn";
+      break;
     }
-    k_igemm_kmajor_bn<BN, STAGES><<<kmajor_grid(p), kThreads, smem, s>>>(amaps, bmap, omap, p, *rmap, *ep);
-    RIGL_LAUNCH_CHECK("k_igemm_kmajor_bn");
-    return RIGL_OK;
+    case ConvEpilogue::kRelu:
+      RIGL_CUDA(smem_limit<k_igemm_kmajor_relu<BN, STAGES, false>>(smem));
+      k_igemm_kmajor_relu<BN, STAGES, false><<<grid, kThreads, smem, s>>>(amaps, bmap, omap, p, rmap);
+      name = "k_igemm_kmajor_relu";
+      break;
+    case ConvEpilogue::kReluGate:
+      RIGL_CUDA(smem_limit<k_igemm_kmajor_relu<BN, STAGES, true>>(smem));
+      k_igemm_kmajor_relu<BN, STAGES, true><<<grid, kThreads, smem, s>>>(amaps, bmap, omap, p, rmap);
+      name = "k_igemm_kmajor_relu";
+      break;
+    default:
+      RIGL_CUDA(smem_limit<k_igemm_kmajor<BN, STAGES>>(smem));
+      k_igemm_kmajor<BN, STAGES><<<grid, kThreads, smem, s>>>(amaps, bmap, omap, p);
+      name = "k_igemm_kmajor";
   }
-  static bool configured = false;
-  if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_kmajor<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
-  k_igemm_kmajor<BN, STAGES><<<kmajor_grid(p), kThreads, smem, s>>>(amaps, bmap, omap, p);
-  RIGL_LAUNCH_CHECK("k_igemm_kmajor");
+  RIGL_LAUNCH_CHECK(name);
   return RIGL_OK;
 }
 
 static int dispatch_kmajor(int n_out, const TMaps4& amaps, const CUtensorMap& bmap, const CUtensorMap& omap,
-                           IgemmParams& p, int bn_tile, cudaStream_t s, const CUtensorMap* rmap = nullptr,
-                           const BnEpilogue* ep = nullptr, int relu = kReluNone) {
+                           IgemmParams& p, int bn_tile, const ConvEpilogue& epi, const CUtensorMap& rmap,
+                           cudaStream_t s) {
   p.n_tiles = (n_out + bn_tile - 1) / bn_tile;
-  if (bn_tile == 64) return launch_kmajor<64, 7>(amaps, bmap, omap, p, s, rmap, ep, relu);
-  return launch_kmajor<128, 5>(amaps, bmap, omap, p, s, rmap, ep, relu);
+  if (bn_tile == 64) return launch_kmajor<64, 7>(amaps, bmap, omap, p, epi, rmap, s);
+  return launch_kmajor<128, 5>(amaps, bmap, omap, p, epi, rmap, s);
 }
 
 static int pick_bn(int n_out) {
@@ -890,51 +933,27 @@ static int pick_bn(int n_out) {
 
 void tc_set_bn_stats_always(bool on) { g_bn_stats_always = on; }
 
-int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, float* y_f32, const float* bias,
-             void* ws, size_t ws_bytes, cudaStream_t s, float* bn_partial, int* bn_rows, const BnApplyArgs* bn_apply,
-             bool relu) {
-  (void)ws; (void)ws_bytes;
+int tc_fprop(const ConvGeom& g, int path, const void* x, const void* packed, void* y, const ConvEpilogue& epi,
+             cudaStream_t s) {
   int rc = ensure_driver();
   if (rc != RIGL_OK) return rc;
   const PackedLayout L = packed_layout(g.taps(), g.cin, g.cout);
   const uint8_t* pk = static_cast<const uint8_t*>(packed);
-  {
+  if (path == kPathHalo) {
     HaloParams hp = {};
-    if (y != nullptr && y_f32 == nullptr && bias == nullptr && halo_fprop_ok(g, &hp)) {
-      if (relu)
-        return halo_launch_kmajor(hp, x, g.cin, g.x_pitch, pk + L.off_fprop, L.cin_pad, g.cout, y, g.cout, false, s,
-                                  true);
-      if (bn_apply != nullptr) {          // no batch-norm epilogue on the halo kernels: plain call + rigl_bn_apply
-        set_error("fused BN apply: layer runs on the halo kernels");
-        return RIGL_ERR_UNSUPPORTED;
-      }
-      if (bn_partial != nullptr) {        // the halo kernels have no statistics epilogue: the caller runs the plain
-        set_error("fused BN statistics: layer runs on the halo kernels");   // call + the stats pass instead
-        return RIGL_ERR_UNSUPPORTED;
-      }
-      return halo_launch_kmajor(hp, x, g.cin, g.x_pitch, pk + L.off_fprop, L.cin_pad, g.cout, y, g.cout, false, s);
-    }
-  }
-  if (bn_partial != nullptr && !g_bn_stats_always) {
-    // The statistics are free when the tile's main loop is long enough to hide them (reduction length
-    // K = taps * cin >= 512), and cost about what the separate stats pass costs -- or more -- for the short-K /
-    // wide-output layers whose epilogue is the bottleneck (1x1 convs with K <= 128; K = 256 with more than 128
-    // output channels).
-    const int K = g.taps() * g.cin;
-    if (!(K >= 512 || (K >= 256 && g.cout <= 128))) {
-      set_error("fused BN statistics: not profitable for this shape (K = %d, cout = %d)", K, g.cout);
-      return RIGL_ERR_UNSUPPORTED;
-    }
+    halo_fprop_ok(g, &hp);            // (true: conv_route chose the halo kernels)
+    return halo_launch_kmajor(hp, x, g.cin, g.x_pitch, pk + L.off_fprop, L.cin_pad, g.cout, y, g.cout, false, s,
+                              epi.kind == ConvEpilogue::kRelu);
   }
   IgemmParams p = {};
   set_pixel_tiling(p, g.out_w, g.out_h, g.batch, 128);
   p.kblks = (g.cin + kBK - 1) / kBK;
   p.N = g.cout;
-  p.out_bf16 = static_cast<__nv_bfloat16*>(y); p.out_f32 = y_f32; p.bias = bias;
+  p.out_bf16 = static_cast<__nv_bfloat16*>(y); p.out_f32 = epi.out_f32; p.bias = epi.bias;
   p.o_off = 0; p.o_sw = g.cout; p.o_sh = (long long)g.out_w * g.cout; p.o_sn = (long long)g.out_h * g.out_w * g.cout;
   p.nnz = reinterpret_cast<const uint32_t*>(pk + L.off_nnz);
   p.nnz_tap_stride = L.n_tiles * L.k_tiles; p.nnz_n_stride = L.k_tiles; p.nnz_k_stride = 1;
-  p.bn_partial = bn_partial;            // (decides the kernel variant, hence the B box: set before the maps)
+  p.bn_partial = epi.bn_partial;
   TMaps4 amaps;
   const uint32_t abox[4] = {(uint32_t)kBK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
   rc = set_conv_taps(p, &amaps, g, x, abox);
@@ -947,50 +966,34 @@ int tc_fprop(const ConvGeom& g, const void* x, const void* packed, void* y, floa
   rc = make_tmap(&bmap, pk + L.off_fprop, 3, bdims, bstr, bbox);
   if (rc != RIGL_OK) return rc;
   CUtensorMap omap = bmap;
-  p.tma_store = (y != nullptr && y_f32 == nullptr && bias == nullptr) ? 1 : 0;
+  p.tma_store = (y != nullptr && epi.out_f32 == nullptr && epi.bias == nullptr) ? 1 : 0;
   if (p.tma_store) {
     rc = make_act_map(&omap, y, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
     if (rc != RIGL_OK) return rc;
   }
-  if (bn_partial) {
-    p.bn_partial = bn_partial;
+  if (epi.kind == ConvEpilogue::kBnStats && epi.bn_rows) {
     p.n_tiles = (g.cout + bn_tile - 1) / bn_tile;
-    if (bn_rows) *bn_rows = kmajor_grid(p);
+    *epi.bn_rows = kmajor_grid(p);
   }
-  if (bn_apply) {
-    CUtensorMap rmap = omap;
-    if (bn_apply->residual) {            // the residual through the output's view: same boxes, same swizzle
-      rc = make_act_map(&rmap, bn_apply->residual, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
-      if (rc != RIGL_OK) return rc;
-    }
-    const BnEpilogue ep = {bn_apply->scale, bn_apply->shift, bn_apply->relu ? 1 : 0, bn_apply->residual ? 1 : 0};
-    return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s, &rmap, &ep);
+  CUtensorMap rmap = omap;
+  if (epi.kind == ConvEpilogue::kBnApply && epi.residual) {   // the residual through the output's view
+    rc = make_act_map(&rmap, epi.residual, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, abox);
+    if (rc != RIGL_OK) return rc;
   }
-  if (relu) return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s, nullptr, nullptr, kReluFprop);
-  return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, s);
+  return dispatch_kmajor(g.cout, amaps, bmap, omap, p, bn_tile, epi, rmap, s);
 }
 
-int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, void* ws, size_t ws_bytes,
-             cudaStream_t s, const void* gate) {
-  (void)ws; (void)ws_bytes;
+int tc_dgrad(const ConvGeom& g, int path, const void* dy, const void* packed, void* dx, const ConvEpilogue& epi,
+             cudaStream_t s) {
   int rc = ensure_driver();
   if (rc != RIGL_OK) return rc;
   const PackedLayout L = packed_layout(g.taps(), g.cin, g.cout);
   const uint8_t* pk = static_cast<const uint8_t*>(packed);
   const int st = g.stride;
-  {
+  if (path == kPathHalo) {
     HaloParams hp = {};
-    if (halo_dgrad_ok(g, &hp)) {
-      if (gate != nullptr) {             // no gated epilogue on the halo kernels: plain call + rigl_relu_gate
-        set_error("gated dgrad: layer runs on the halo kernels");
-        return RIGL_ERR_UNSUPPORTED;
-      }
-      return halo_launch_kmajor(hp, dy, g.cout, g.cout, pk + L.off_dgrad, L.cout_pad, g.cin, dx, g.x_pitch, true, s);
-    }
-  }
-  if (gate != nullptr && st != 1) {
-    set_error("gated dgrad: only the single-launch stride-1 dgrad has the gate");
-    return RIGL_ERR_UNSUPPORTED;
+    halo_dgrad_ok(g, &hp);            // (true: conv_route chose the halo kernels)
+    return halo_launch_kmajor(hp, dy, g.cout, g.cout, pk + L.off_dgrad, L.cout_pad, g.cin, dx, g.x_pitch, true, s);
   }
   // classes of input pixels by parity; each class is one launch over its sub-grid
   bool need_zero = false;
@@ -1039,15 +1042,12 @@ int tc_dgrad(const ConvGeom& g, const void* dy, const void* packed, void* dx, vo
       rc = make_act_map(&omap, dx, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
       if (rc != RIGL_OK) return rc;
       p.tma_store = 1;
-      if (gate != nullptr) {            // x through dx's view: the gate box is the output box
-        CUtensorMap xmap;
-        rc = make_act_map(&xmap, gate, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
+      CUtensorMap rmap = omap;
+      if (epi.kind == ConvEpilogue::kReluGate) {   // x through dx's view: the gate box is the output box
+        rc = make_act_map(&rmap, epi.gate, g.batch, g.in_h, g.in_w, g.cin, g.x_pitch, st, ph, pw, abox);
         if (rc != RIGL_OK) return rc;
-        rc = dispatch_kmajor(g.cin, amaps, bmap, omap, p, bn_tile, s, &xmap, nullptr, kReluGateDgrad);
-        if (rc != RIGL_OK) return rc;
-        continue;
       }
-      rc = dispatch_kmajor(g.cin, amaps, bmap, omap, p, bn_tile, s);
+      rc = dispatch_kmajor(g.cin, amaps, bmap, omap, p, bn_tile, epi, rmap, s);
       if (rc != RIGL_OK) return rc;
     }
   return RIGL_OK;
@@ -1057,11 +1057,7 @@ template <int BN, int STAGES>
 static int launch_wgrad(const TMaps4& xmaps, const CUtensorMap& dymap, const WgradParams& p, cudaStream_t s) {
   constexpr size_t smem = (size_t)STAGES * (kBM * kBK * 2 + BN * kBK * 2) + 1024 + 256;
   static_assert(smem <= 227 * 1024, "wgrad kernel exceeds the shared memory of an SM");
-  static bool configured = false;
-  if (!configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_igemm_wgrad<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
+  RIGL_CUDA(smem_limit<k_igemm_wgrad<BN, STAGES>>(smem));
   const int units = p.ntaps * p.m_tiles * p.n_tiles * p.splits;
   const int grid = units < g_num_sms ? units : g_num_sms;
   k_igemm_wgrad<BN, STAGES><<<grid, kThreads, smem, s>>>(xmaps, dymap, p);
@@ -1069,27 +1065,26 @@ static int launch_wgrad(const TMaps4& xmaps, const CUtensorMap& dymap, const Wgr
   return RIGL_OK;
 }
 
-int tc_wgrad(const ConvGeom& g, const void* x, const void* dy, float* dw, float beta, void* ws, size_t ws_bytes,
-             cudaStream_t s) {
+int tc_wgrad(const ConvGeom& g, int path, const void* x, const void* dy, float* dw, float beta, void* ws,
+             size_t ws_bytes, cudaStream_t s) {
   int rc = ensure_driver();
   if (rc != RIGL_OK) return rc;
-  {
+  if (path == kPathHalo) {
     HaloParams hp = {};
-    if (halo_wgrad_ok(g, &hp)) {
-      const size_t need = halo_wgrad_ws_elems(g, hp) * sizeof(float);
-      float* wsf = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
-      if (ws == nullptr || ws_bytes < need + 256) {
-        set_error("rigl_conv2d_wgrad_dense: workspace %zu < required %zu", ws_bytes, need + 256);
-        return RIGL_ERR_WORKSPACE;
-      }
-      rc = halo_launch_wgrad(hp, g, x, dy, wsf, s);
-      if (rc != RIGL_OK) return rc;
-      const long long n_w9 = (long long)9 * g.cin * g.cout;
-      const long long threads = (n_w9 + 3) / 4;
-      k_splitk_reduce<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(wsf, n_w9, halo_wgrad_grid(hp), dw, n_w9, beta);
-      RIGL_LAUNCH_CHECK("k_splitk_reduce");
-      return RIGL_OK;
+    halo_wgrad_ok(g, &hp);            // (true: conv_route chose the halo kernels)
+    const size_t need = halo_wgrad_ws_elems(g, hp) * sizeof(float);
+    float* wsf = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
+    if (ws == nullptr || ws_bytes < need + 256) {
+      set_error("rigl_conv2d_wgrad_dense: workspace %zu < required %zu", ws_bytes, need + 256);
+      return RIGL_ERR_WORKSPACE;
     }
+    rc = halo_launch_wgrad(hp, g, x, dy, wsf, s);
+    if (rc != RIGL_OK) return rc;
+    const long long n_w9 = (long long)9 * g.cin * g.cout;
+    const long long threads = (n_w9 + 3) / 4;
+    k_splitk_reduce<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(wsf, n_w9, halo_wgrad_grid(hp), dw, n_w9, beta);
+    RIGL_LAUNCH_CHECK("k_splitk_reduce");
+    return RIGL_OK;
   }
   WgradParams p = {};
   set_pixel_tiling(p, g.out_w, g.out_h, g.batch, 64);

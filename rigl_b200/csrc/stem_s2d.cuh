@@ -370,11 +370,7 @@ int s2d_fprop(const ConvGeom& g, const void* xs, const void* packed, void* y, cu
   rc = make_act_map(&omap, y, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, obox);
   if (rc != RIGL_OK) return rc;
   const size_t smem = 16 * kS2dBTapBytes + p.nbuf * (size_t)p.a_buf_bytes + 2 * (128 * 64 * 2) + 1024 + 256;
-  static size_t configured = 0;
-  if (smem > configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_stem_s2d_fprop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
+  RIGL_CUDA(smem_limit<k_stem_s2d_fprop>(smem));
   const int sms = g_num_sms > 0 ? g_num_sms : kNumSmsHint;
   const dim3 grid(p.total_strips < sms ? p.total_strips : sms, p.groups);
   k_stem_s2d_fprop<<<grid, kThreads, smem, s>>>(amap, bmap, omap, p);
@@ -402,11 +398,7 @@ int s2d_wgrad(const ConvGeom& g, const void* xs, const void* dy, float* dw, floa
   rc = make_act_map(&dymap, dy, g.batch, g.out_h, g.out_w, g.cout, g.cout, 1, 0, 0, dbox);
   if (rc != RIGL_OK) return rc;
   const size_t smem = p.nbuf * ((size_t)p.a_buf_bytes + (size_t)p.R * kS2dWp * 128) + 1024 + 256;
-  static size_t configured = 0;
-  if (smem > configured) {
-    RIGL_CUDA(cudaFuncSetAttribute(k_stem_s2d_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
+  RIGL_CUDA(smem_limit<k_stem_s2d_wgrad>(smem));
   k_stem_s2d_wgrad<<<dim3(grid, p.groups), kThreads, smem, s>>>(xmap, dymap, p);
   RIGL_LAUNCH_CHECK("k_stem_s2d_wgrad");
   const int total = g.ksize * g.ksize * g.cin * g.cout;

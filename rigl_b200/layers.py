@@ -90,6 +90,16 @@ def relu_gate(x, g, out):
   return out
 
 
+def _run_fused(name, *args):
+  """Calls the fused conv entry point `name`: True once it has launched, False where it returned RIGL_ERR_UNSUPPORTED
+  (the layer's kernel has no such epilogue; nothing launched, the caller runs the unfused form).  Other errors raise."""
+  rc = getattr(_cabi.lib(), name)(*args)
+  if rc == _cabi.RIGL_ERR_UNSUPPORTED:
+    return False
+  _cabi.check(rc, name)
+  return True
+
+
 def _workspace(device, nbytes):
   key = (device, _WS_SLOT[0])          # one scratch buffer per (device, stream role)
   ws = _WS.get(key)
@@ -473,39 +483,28 @@ class SparseConv2d(_MaskedLayer):
       self._patch_cache = src = self._patches(x)
       d, packed = self._patch_desc(src.shape[0]), self.packed_patch
     ws = _workspace(x.device, _cabi.lib().rigl_conv_workspace_bytes(d))
+    conv, tail = (d, src.data_ptr(), packed.data_ptr()), (ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
+
+    def plain(y_bf16, y_f32):
+      _cabi.check(_cabi.lib().rigl_masked_conv2d_fprop(*conv, y_bf16, y_f32, None, *tail), 'rigl_masked_conv2d_fprop')
+
     if out_f32:           # (a masked classifier in conv form, VGG's fc8): fp32 logits
-      _cabi.check(_cabi.lib().rigl_masked_conv2d_fprop(
-          d, src.data_ptr(), packed.data_ptr(), None, y.data_ptr(), None, ws.data_ptr(), ws.numel(),
-          _cabi.stream_ptr()), 'rigl_masked_conv2d_fprop')
+      plain(None, y.data_ptr())
       return y
     if self.relu_out:
-      if FUSE_RELU:
-        rc = _cabi.lib().rigl_masked_conv2d_fprop_relu(d, src.data_ptr(), packed.data_ptr(), y.data_ptr(),
-                                                       ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
-        if rc == 0:
-          return y
-        if rc != -4:      # RIGL_ERR_UNSUPPORTED (nothing launched): plain call + the standalone gate
-          _cabi.check(rc, 'rigl_masked_conv2d_fprop_relu')
-      _cabi.check(_cabi.lib().rigl_masked_conv2d_fprop(
-          d, src.data_ptr(), packed.data_ptr(), y.data_ptr(), None, None, ws.data_ptr(),
-          ws.numel(), _cabi.stream_ptr()), 'rigl_masked_conv2d_fprop')
-      return relu_gate(y, y, y)
+      if not (FUSE_RELU and _run_fused('rigl_masked_conv2d_fprop_relu', *conv, y.data_ptr(), *tail)):
+        plain(y.data_ptr(), None)       # unfused: plain call + the standalone gate
+        relu_gate(y, y, y)
+      return y
     self.bn_partial = None
     if self.collect_bn_stats and self.training and FUSE_BN_STATS:
       # the epilogue also emits per-CTA column sums / sums of squares of the output (BN statistics)
       rows = C.c_int(0)
       part = torch.empty(_bn_partial_rows() * 2 * self._cout, dtype=torch.float32, device=x.device)
-      rc = _cabi.lib().rigl_masked_conv2d_fprop_bnstats(
-          d, src.data_ptr(), packed.data_ptr(), y.data_ptr(), part.data_ptr(), C.byref(rows), ws.data_ptr(),
-          ws.numel(), _cabi.stream_ptr())
-      if rc == 0:
+      if _run_fused('rigl_masked_conv2d_fprop_bnstats', *conv, y.data_ptr(), part.data_ptr(), C.byref(rows), *tail):
         self.bn_partial = (part, rows.value, y.data_ptr())
         return y
-      if rc != -4:        # RIGL_ERR_UNSUPPORTED: fall through to the plain call
-        _cabi.check(rc, 'rigl_masked_conv2d_fprop_bnstats')
-    _cabi.check(_cabi.lib().rigl_masked_conv2d_fprop(
-        d, src.data_ptr(), packed.data_ptr(), y.data_ptr(), None, None, ws.data_ptr(),
-        ws.numel(), _cabi.stream_ptr()), 'rigl_masked_conv2d_fprop')
+    plain(y.data_ptr(), None)
     return y
 
   def _dgrad(self, dy, x):
@@ -515,17 +514,14 @@ class SparseConv2d(_MaskedLayer):
       super(SparseConv2d, self).pack()
     dx = torch.empty_like(x, memory_format=torch.channels_last)
     ws = _workspace(x.device, _cabi.lib().rigl_conv_workspace_bytes(d))
-    if self.gate_dgrad and FUSE_RELU:
-      rc = _cabi.lib().rigl_masked_conv2d_dgrad_relu(d, dy.data_ptr(), self.packed.data_ptr(), x.data_ptr(),
-                                                     dx.data_ptr(), ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
-      if rc == 0:
-        return dx
-      if rc != -4:        # RIGL_ERR_UNSUPPORTED (nothing launched): plain call + the standalone gate
-        _cabi.check(rc, 'rigl_masked_conv2d_dgrad_relu')
+    if self.gate_dgrad and FUSE_RELU and _run_fused(
+        'rigl_masked_conv2d_dgrad_relu', d, dy.data_ptr(), self.packed.data_ptr(), x.data_ptr(), dx.data_ptr(),
+        ws.data_ptr(), ws.numel(), _cabi.stream_ptr()):
+      return dx
     _cabi.check(_cabi.lib().rigl_masked_conv2d_dgrad(
         d, dy.data_ptr(), self.packed.data_ptr(), dx.data_ptr(), ws.data_ptr(), ws.numel(),
         _cabi.stream_ptr()), 'rigl_masked_conv2d_dgrad')
-    return relu_gate(x, dx, dx) if self.gate_dgrad else dx
+    return relu_gate(x, dx, dx) if self.gate_dgrad else dx     # unfused: plain call + the standalone gate
 
   def _wgrad(self, x, dy, out, accumulate):
     n, c, h, w = x.shape
@@ -564,13 +560,11 @@ class SparseConv2d(_MaskedLayer):
     if residual is not None and residual.shape != out.shape:
       raise ValueError('residual of shape %s for an output of shape %s' % (tuple(residual.shape), tuple(out.shape)))
     ws = _workspace(x.device, _cabi.lib().rigl_conv_workspace_bytes(d))
-    rc = _cabi.lib().rigl_masked_conv2d_fprop_bnapply(
-        d, x.data_ptr(), self.packed.data_ptr(), None if residual is None else residual.data_ptr(), scale.data_ptr(),
-        shift.data_ptr(), int(bn.relu), out.data_ptr(), ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
-    if rc == -4:          # RIGL_ERR_UNSUPPORTED (nothing launched)
-      return None
-    _cabi.check(rc, 'rigl_masked_conv2d_fprop_bnapply')
-    return out
+    fused = _run_fused(
+        'rigl_masked_conv2d_fprop_bnapply', d, x.data_ptr(), self.packed.data_ptr(),
+        None if residual is None else residual.data_ptr(), scale.data_ptr(), shift.data_ptr(), int(bn.relu),
+        out.data_ptr(), ws.data_ptr(), ws.numel(), _cabi.stream_ptr())
+    return out if fused else None
 
   def forward(self, x, bn=None, residual=None):
     """conv(x), or with `bn` (a FusedBatchNormReLU over this layer's output) bn(conv(x), residual): in the

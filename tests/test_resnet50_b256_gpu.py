@@ -3,7 +3,7 @@
 
 Covered: every distinct masked layer of workloads.ResNet50 -- the space-to-depth stem (csrc/stem_s2d.cuh), the 22
 distinct conv shapes and final_dense -- run as the model trains them: train mode, bf16 channels_last input, fprop
-with the batch-norm statistics epilogue where the model asks for it and the policy of tc_fprop grants it, then
+with the batch-norm statistics epilogue where the model asks for it and the policy of conv_route grants it, then
 dgrad (not for the stem: the image needs no gradient) and the dense wgrad through the layer's autograd function.
 At this size the launchers take decisions nothing smaller reaches: the stem's wgrad runs 7168 strips over one CTA
 per SM (~55 strips, 24 k positions accumulated in fp32 per CTA) and adds the 132 partials in k_stem_s2d_reduce;
@@ -122,7 +122,7 @@ def _is_halo(entry):
 
 
 def _stats_epilogue(entry):
-  """tc_fprop's policy for the batch-norm statistics epilogue: the layer asks for it (collect_bn_stats), is not on
+  """conv_route's policy for the batch-norm statistics epilogue: the layer asks for it (collect_bn_stats), is not on
   the halo kernels or the stem's path, and K = taps * cin >= 512, or K >= 256 with cout <= 128."""
   l = entry['layer']
   if entry['kind'] != 'conv' or _is_stem(entry) or _is_halo(entry) or not l.collect_bn_stats:
