@@ -240,6 +240,26 @@ RIGL_API int rigl_adam_plan_destroy(rigl_adam_plan* plan);
 RIGL_API int rigl_adam_plan_run(rigl_adam_plan* plan, const float* lr_dev, float* powers_dev, float beta1, float beta2,
                                 float epsilon, void* stream);
 
+/* Per-step training summaries (imagenet_train_eval.py:431-470: grad_norm, var_norm, fw_nz_*, mask sparsities) over
+ * the parameters of an optimizer plan, on the same task table.  Per element, in float32 as the optimizers form it,
+ *   g = (bit ? grad * grad_scale : 0) + reg_decay * w,
+ * and per parameter, accumulated in float64 from the element on, out_dev[i][5] =
+ *   { sum w^2, sum g^2, sum |w|, count(w != 0) (NaN counts, +-0 does not), set bits of mask_bits (0 when NULL) }.
+ * run: two launches on `stream` (per-task partial rows, then each parameter's rows added in task order), no
+ * synchronisation; the result is bit-identical run to run.  The plan owns the partial rows: one run at a time. */
+typedef struct {
+  const float* param;          /* [n] raw weights */
+  const float* grad;           /* [n] gradient; the DENSE gradient when mask_bits != NULL */
+  const uint32_t* mask_bits;   /* NULL (dense parameter) or the layer's bitmap */
+  int64_t n;
+  float grad_scale;            /* multiplies grad (1/replicas for the summed gradients) */
+  float reg_decay;             /* l2 coefficient of the summarised loss (0: not regularized) */
+} rigl_summary_desc;
+typedef struct rigl_summary_plan rigl_summary_plan;
+RIGL_API int rigl_summary_plan_create(const rigl_summary_desc* params, int n_params, rigl_summary_plan** out);
+RIGL_API int rigl_summary_plan_destroy(rigl_summary_plan* plan);
+RIGL_API int rigl_summary_plan_run(rigl_summary_plan* plan, double* out_dev, void* stream);
+
 /* ------------------------------------------------------------------------
  * Masked conv2d / linear as implicit GEMM (wgmma on sm_90a; a CUDA-core
  * kernel serves shapes whose row pitch is not a 16-byte multiple).

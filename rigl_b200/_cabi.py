@@ -14,7 +14,7 @@ _lib = None
 # residual form without a ReLU bitmap when relu == 0 (the linear bottleneck of MobileNet-v2).  Library version 203
 # only adds rigl_masked_conv2d_fprop_bnapply; no calling rule of an existing symbol changed, and a library without
 # the new symbol already fails its lookup in lib().  204 only adds the ReLU entry points (conv epilogues, the 2x2
-# pool, rigl_relu_gate), likewise; 205 only adds rigl_mask_prune_run.
+# pool, rigl_relu_gate), likewise; 205 only adds rigl_mask_prune_run; 206 only adds rigl_summary_plan_*.
 ABI_VERSION = 202
 
 
@@ -42,6 +42,11 @@ class SgdDesc(C.Structure):
 class AdamDesc(C.Structure):
   _fields_ = [('param', C.c_void_p), ('m', C.c_void_p), ('v', C.c_void_p), ('grad', C.c_void_p),
               ('mask_bits', C.c_void_p), ('n', C.c_int64), ('weight_decay', C.c_float), ('grad_scale', C.c_float)]
+
+
+class SummaryDesc(C.Structure):
+  _fields_ = [('param', C.c_void_p), ('grad', C.c_void_p), ('mask_bits', C.c_void_p), ('n', C.c_int64),
+              ('grad_scale', C.c_float), ('reg_decay', C.c_float)]
 
 
 class ConvDesc(C.Structure):
@@ -87,6 +92,9 @@ SIGNATURES = {
     'rigl_adam_plan_create': (C.c_int, [C.POINTER(AdamDesc), _i32, C.POINTER(_vp)]),
     'rigl_adam_plan_destroy': (C.c_int, [_vp]),
     'rigl_adam_plan_run': (C.c_int, [_vp, _vp, _vp, _f32, _f32, _f32, _vp]),
+    'rigl_summary_plan_create': (C.c_int, [C.POINTER(SummaryDesc), _i32, C.POINTER(_vp)]),
+    'rigl_summary_plan_destroy': (C.c_int, [_vp]),
+    'rigl_summary_plan_run': (C.c_int, [_vp, _vp, _vp]),
     'rigl_conv_workspace_bytes': (_sz, [C.POINTER(ConvDesc)]),
     'rigl_masked_conv2d_fprop': (C.c_int, [C.POINTER(ConvDesc), _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     'rigl_bn_partial_rows': (C.c_int, []),

@@ -80,15 +80,11 @@ class _FusedInnerOptimizer(torch.optim.Optimizer):
     """Device buffers the plan's launches read besides the per-parameter ones."""
     return ()
 
-  @torch.no_grad()
-  def prepare(self):
-    """Creates the slots, the device learning rate and the launch plan for the CURRENT gradient
-    buffers.  Allocates, so it cannot run under stream capture: call it once before capturing `step()`
-    (TrainHarness.enable_cuda_graph does)."""
-    g = self.param_groups[0]
-    self._upload_lr()
-    ents = []
-    for p in g['params']:
+  def plan_params(self):
+    """(param, grad, bitmap or None, grad_scale) of every parameter the next step updates, in plan order: a masked
+    layer's weight with its dense gradient and bitmap, every other parameter that has a `.grad`."""
+    out = []
+    for p in self.param_groups[0]['params']:
       layer = self._masked.get(id(p))
       if layer is not None:
         grad, bits, scale = layer.masked_weights.dense_grad, layer.mask.bits, self._grad_scale
@@ -99,8 +95,20 @@ class _FusedInnerOptimizer(torch.optim.Optimizer):
       if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous() or grad.dtype != torch.float32 \
           or not grad.is_contiguous():
         raise ValueError('%s needs contiguous float32 CUDA parameters and gradients' % self._name)
+      out.append((p, grad, bits, float(scale)))
+    return out
+
+  @torch.no_grad()
+  def prepare(self):
+    """Creates the slots, the device learning rate and the launch plan for the CURRENT gradient
+    buffers.  Allocates, so it cannot run under stream capture: call it once before capturing `step()`
+    (TrainHarness.enable_cuda_graph does)."""
+    g = self.param_groups[0]
+    self._upload_lr()
+    ents = []
+    for p, grad, bits, scale in self.plan_params():
       ents.append((p.data_ptr(), tuple(s.data_ptr() for s in self._slots(p)), grad.data_ptr(),
-                   0 if bits is None else bits.data_ptr(), p.numel(), float(g['weight_decay']), float(scale)))
+                   0 if bits is None else bits.data_ptr(), p.numel(), float(g['weight_decay']), scale))
     key = (tuple(ents), self._plan_extra_key())
     if key != self._key:
       self._destroy()

@@ -579,7 +579,7 @@ class TrainHarness(object):
   def __init__(self, model, lr=0.1, momentum=0.9, weight_decay=1e-4, label_smoothing=0.1,
                drop_fraction=0.3, drop_fraction_anneal='cosine', begin_step=0, end_step=25000,
                frequency=100, data_parallel=None, optimizer_cls=SparseRigLOptimizer, lr_schedule=None,
-               fused_optimizer=None, inner_optimizer='momentum', pruning=None):
+               fused_optimizer=None, inner_optimizer='momentum', pruning=None, summaries=False):
     """lr_schedule: optional callable(global_step) -> learning rate, evaluated on the host before every step
     (optim.make_imagenet_lr_fn is the reference's, imagenet_train_eval.py:317-354); `lr` is then only the
     initial value.  fused_optimizer: the inner optimizer is optim.FusedMomentumSGD (one launch, mask * dense_grad
@@ -589,7 +589,10 @@ class TrainHarness(object):
     the constant base_lr * batch / 256).  'adam' exists only on the fused path: `momentum` is then unused.
     optimizer_cls=None: the inner optimizer alone, one step and one global-step increment per step (the
     reference's scratch / baseline / prune methods: `optimizer.minimize`).  pruning: a pruning.Pruning whose
-    conditional_mask_update_op() runs after every step, eager or graphed; it counts this harness's global step."""
+    conditional_mask_update_op() runs after every step, eager or graphed; it counts this harness's global step.
+    summaries: every step also reduces the reference's per-step training scalars (summaries.TrainSummaries: two
+    launches after the gradient exchange, before the optimizer or mask update); `summaries()` reads the last step's.
+    Needs the fused inner optimizer."""
     import os
     if inner_optimizer not in ('momentum', 'adam'):
       raise ValueError("inner_optimizer must be 'momentum' or 'adam', got %r" % (inner_optimizer,))
@@ -635,6 +638,10 @@ class TrainHarness(object):
       if self.dp is not None:
         self.dp.masked_grads_in_optimizer = True
         self.dp.other_scale_in_optimizer = True
+    self._summaries, self._last_summary = None, None
+    if summaries:
+      from .summaries import TrainSummaries
+      self._summaries = TrainSummaries(model, self.inner)
 
   def _apply_lr_schedule(self):
     if self.lr_schedule is None:
@@ -648,6 +655,31 @@ class TrainHarness(object):
                            'with an lr schedule')
       for g in self.inner.param_groups:
         g['lr'] = lr
+
+  def _launch_summaries(self):
+    """After the gradient exchange, before any optimizer or mask update, so the reduction reads the state the
+    step's loss was computed at.  Returns the step's (global step, learning rate), or None without summaries."""
+    if self._summaries is None:
+      return None
+    self._summaries.run()
+    return self.global_step.value, float(self.inner.param_groups[0]['lr'])
+
+  def _record_summary(self, head, loss):
+    if head is not None:
+      from .sparse_optimizers_base import SparseSETOptimizerBase
+      # is_mask_update_iter set it for this step (0 off update steps)
+      drop = self.opt.drop_fraction if isinstance(self.opt, SparseSETOptimizerBase) else None
+      self._last_summary = head + (loss.detach(), drop)      # (holding the autograd graph would break a capture)
+
+  def summaries(self):
+    """The last step's training summaries as a dict of floats (DESIGN.md 5 defines each key), after one device
+    synchronisation.  Raises RuntimeError when the harness was built without summaries or no step has run."""
+    if self._summaries is None:
+      raise RuntimeError('this TrainHarness was built without summaries (TrainHarness(..., summaries=True))')
+    if self._last_summary is None:
+      raise RuntimeError('TrainHarness.summaries() before the first step')
+    gs, lr, loss, drop = self._last_summary
+    return self._summaries.read(loss, gs, lr, drop)
 
   # ---- CUDA-graph mode: the forward+backward and the inner optimizer step are captured once and
   # replayed (inter-kernel launch gaps and all host work disappear); the data-parallel
@@ -729,6 +761,7 @@ class TrainHarness(object):
     self.replayed_kernel_launches += self.graph_kernel_launches
     if self.dp is not None:
       self.dp.reduce_gradients(self.model)
+    head = self._launch_summaries()
     gs = self.global_step
     def inner_step():
       self._g_opt.replay()
@@ -742,6 +775,7 @@ class TrainHarness(object):
       self.opt.cond_mask_update_op(gs, inner_step)
     if self.pruning is not None:
       self.pruning.conditional_mask_update_op()
+    self._record_summary(head, self._sloss)
     return self._sloss
 
   def step(self, images, labels):
@@ -754,6 +788,7 @@ class TrainHarness(object):
     loss = self._forward_backward(images, labels, set_to_none=self.dp is None)
     if self.dp is not None:
       self.dp.reduce_gradients(self.model)
+    head = self._launch_summaries()
     if self.opt is None:
       self.inner.step()
       self.global_step.increment()
@@ -762,6 +797,7 @@ class TrainHarness(object):
       self.opt.apply_gradients(None, global_step=self.global_step)
     if self.pruning is not None:
       self.pruning.conditional_mask_update_op()
+    self._record_summary(head, loss)
     return loss
 
 
